@@ -1,7 +1,7 @@
 """`import assistive_gym` drop-in for the reference package (reference assistive_gym/__init__.py:1-33).
 
 Registers the `-v1` ids this backend has built with gym (when gym is importable), exactly as the reference does, so that
-`gym.make('assistive_gym:FeedingJaco-v1')` and `learn.py:61-69 make_env` resolve to the B200 batched backend with
+`gym.make('assistive_gym:FeedingJaco-v1')` and `learn.py:61-69 make_env` resolve to the H100 batched backend with
 `n_envs=1`; `assistive_gym.make(id, n_envs=...)` gives the batched env without gym.  Ids the backend has not built
 raise the registry's KeyError (nothing is silently substituted)."""
 from assistive_gym_b200.envs import ENV_REGISTRY, make  # noqa: F401

@@ -9,11 +9,11 @@
 //   position solver: piterations x [anchors (kAHR), rigid contacts (kCHR / kKHR, kDF), links (kLST) in list order]
 //   velocities:      v = (x - q) / dt * (1 - kDP)
 // Multibody link colliders are not btRigidBody, so Bullet of the reference's era treats them as static shapes with zero
-// velocity: the coupling is one way (cloth feels the bodies, bodies do not feel the cloth).  That is what makes the B200
+// velocity: the coupling is one way (cloth feels the bodies, bodies do not feel the cloth).  That is what makes the GPU
 // mapping below possible: the rigid substeps of one stepSimulation run first and leave the link poses of every substep in
 // a snapshot buffer; ONE launch of k_cloth then advances the cloth through all numSubSteps substeps.
 //
-// B200 mapping.  One CTA of 1024 threads per env, the env's node positions resident in shared memory as float4 (64 KB) for
+// GPU mapping.  One CTA of 1024 threads per env, the env's node positions resident in shared memory as float4 (64 KB) for
 // the whole launch; previous positions q and velocities v of a thread's own nodes (node = k * 1024 + thread) live in its
 // registers.  HBM traffic per env and launch: x and v read once and written once (190 KB) instead of once per substep.
 // Links are relaxed colour by colour (links of one colour share no node; the list is colour-major, so this is the

@@ -1,4 +1,4 @@
-// ag_device.cuh — per-lane bodies of the sm_100a kernels (one env per lane, lock-step).
+// ag_device.cuh — per-lane bodies of the sm_90a kernels (one env per lane, lock-step).
 //
 // Every function here is `__host__ __device__`: the CUDA build wraps them in __global__ kernels
 // (agphys.cu); tests/kernel_harness compiles the same bodies for the host to check kernel logic
@@ -116,7 +116,7 @@ AG_HD bool aabb_ov(f3 amin, f3 amax, f3 bmin, f3 bmax, float m) {
 // closest point on segment / triangle to the origin (barycentric), Ericson RTCD 5.1 — in fp64:
 // the simplex vertices are differences of support points that can be ~1 m apart while the origin is
 // ~1 mm from the simplex; in fp32 the Voronoi-region determinants lose all significance on such thin
-// simplices (measured on B200: 9 % of link-vs-table-edge queries off by up to 2 mm).
+// simplices (measured: 9 % of link-vs-table-edge queries off by up to 2 mm).
 AG_HD void seg_origin(d3 a, d3 b, double& u, double& v) {
   d3 ab = b - a;
   double t = -dot(a, ab), den = dot(ab, ab);

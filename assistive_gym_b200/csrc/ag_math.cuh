@@ -1,4 +1,4 @@
-// ag_math.cuh — fp32 vector / quaternion helpers for the sm_100a kernels.
+// ag_math.cuh — fp32 vector / quaternion helpers for the sm_90a kernels.
 #pragma once
 #include <math.h>
 #include <stdint.h>

@@ -6,7 +6,7 @@
 // rows, implicit cone), solved by projected Gauss-Seidel in that order, 50 iterations, early exit on
 // the least-squares residual.
 //
-// B200 design (round 2).  The Gauss-Seidel chain of one env is strictly sequential, so K7's speed is
+// Design (round 2).  The Gauss-Seidel chain of one env is strictly sequential, so K7's speed is
 // the latency and the instruction count of one row update; round 1 ran it on ONE lane per env
 // (~450 cycles and ~115 warp instructions per row).  Now EIGHT lanes cooperate on an env and a warp
 // carries four envs in lock-step:

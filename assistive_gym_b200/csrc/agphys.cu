@@ -1,6 +1,6 @@
-// agphys.cu — kernels + C ABI (include/agphys.h) of the B200-native batched physics step.
+// agphys.cu — kernels + C ABI (include/agphys.h) of the H100-native batched physics step.
 //
-// Build (product):  nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -shared -Xcompiler -fPIC
+// Build (product):  nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -shared -Xcompiler -fPIC
 // Build (kernel-logic harness, tests only):  g++ -x c++ -DAG_CPU_EMU ...   (never loaded by the package)
 #include <stdio.h>
 #include <stdlib.h>

@@ -12,6 +12,10 @@ Prints ONE JSON line on rank 0.  `value` = device-resident throughput (actions a
 `e2e` = the same metric through the host-buffer C-ABI call (H2D of actions, D2H of obs/reward/done
 inside the timed region), `roofline` = the dominant kernel's algorithmic bytes / measured device
 time against the measured HBM peak, `cpu_baseline` = the oracle timed on a bounded sample.
+
+  --dump-outputs DIR   after the timed steps, write what the timed path returned in its last step (obs, reward, done,
+                       info of rank 0's envs) as DIR/<name>.npy in float32, so that two builds can be compared
+                       output for output: the inputs (start states, actions) depend only on the arguments.
 """
 import argparse
 import json
@@ -39,7 +43,7 @@ def measured_peak():
             return float(json.load(open(p))['hbm_gbs']), 'measured (MEASURED_PEAKS.json)'
         except Exception:
             pass
-    return 6650.0, 'fallback (B200_PROFILING.md)'
+    return 3350.0, 'H100 SXM data sheet (not measured)'
 
 
 class ClockSampler:
@@ -51,8 +55,15 @@ class ClockSampler:
         self.gpu = gpu
         self.lines = []
         self.proc = None
+        self.card = {'gpu': None, 'power_limit_w': None}
 
     def start(self):
+        try:      # what the numbers were measured on: the card's name and its power limit
+            name, plim = subprocess.run(['nvidia-smi', '-i', str(self.gpu), '--query-gpu=name,power.limit', '--format=csv,noheader,nounits'],
+                                        capture_output=True, text=True, timeout=30).stdout.strip().split(', ')[:2]
+            self.card = {'gpu': name, 'power_limit_w': float(plim)}
+        except Exception:
+            pass
         try:
             self.proc = subprocess.Popen(['nvidia-smi', '-i', str(self.gpu), '--query-gpu=' + self.Q, '--format=csv,noheader,nounits', '-lms', '100'],
                                          stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
@@ -67,9 +78,10 @@ class ClockSampler:
 
     def stop(self):
         if self.proc is None:
-            return {'sm_mhz': None, 'sm_max_mhz': None, 'reasons': ['nvidia-smi unavailable']}
+            return dict(self.card, sm_mhz=None, sm_max_mhz=None, reasons=['nvidia-smi unavailable'])
         time.sleep(0.15)
         self.proc.terminate()
+        self.proc.wait()
         sm, mx, reasons = [], [], set()
         for l in self.lines:
             f = [x.strip() for x in l.split(',')]
@@ -83,8 +95,30 @@ class ClockSampler:
             for name, v in zip(('hw_slowdown', 'hw_thermal_slowdown', 'sw_thermal_slowdown', 'sw_power_cap'), f[4:8]):
                 if v.lower().startswith('active'):
                     reasons.add(name)
-        return {'sm_mhz': float(np.median(sm)) if sm else None, 'sm_max_mhz': float(np.max(mx)) if mx else None,
+        return {**self.card, 'sm_mhz': float(np.median(sm)) if sm else None, 'sm_max_mhz': float(np.max(mx)) if mx else None,
                 'reasons': sorted(reasons), 'samples': len(sm)}
+
+
+def dump_outputs(path, arrays, limit=64 << 20):
+    """--dump-outputs: one float32 DIR/<name>.npy per array (leading axis = env).  Above `limit` bytes in all, the same
+    seeded sample of envs is kept from every array and their ids are written as env_index.npy."""
+    arrays = {k: np.asarray(v, dtype=np.float32) for k, v in arrays.items()}
+    n = len(next(iter(arrays.values())))
+    total = sum(a.nbytes for a in arrays.values())
+    if total > limit:
+        keep = np.sort(np.random.default_rng(0).choice(n, size=max(1, int(limit / (total / n + 8))), replace=False))
+        arrays = dict({k: a[keep] for k, a in arrays.items()}, env_index=keep.astype(np.float64))
+    os.makedirs(path, exist_ok=True)
+    for k, a in arrays.items():
+        np.save(os.path.join(path, k + '.npy'), a)
+
+
+def device_mb_since(free0, dev=None):
+    """Device memory taken since `free0` = torch.cuda.mem_get_info()[0] was read, in MiB: the simulation's allocations
+    (cudaMalloc through the C ABI, invisible to torch's allocator statistics) plus the bench's own buffers."""
+    import torch
+    torch.cuda.synchronize(dev)
+    return (free0 - torch.cuda.mem_get_info(dev)[0]) / 2 ** 20
 
 
 def usable_cores():
@@ -192,7 +226,7 @@ def run_reference(args):
 
 
 def run_bedbathing(args):
-    """BASELINE.json configs[2]: BedBathingSawyer-v1 @ batch 4096 on one B200, fused step, from a start pose with the
+    """BASELINE.json configs[2]: BedBathingSawyer-v1 @ batch 4096 on one GPU, fused step, from a start pose with the
     wiping pad 3 mm above the forearm (random joint actions press it onto the skin): device-timed value + host-buffer e2e."""
     import torch
     from assistive_gym_b200 import capi
@@ -203,6 +237,7 @@ def run_bedbathing(args):
         return
     n, K, W = args.batch, args.steps, max(args.warmup, 3)
     bb = BedBathingBatch()
+    free0 = torch.cuda.mem_get_info()[0]
     sim = BatchSim(bb.scene, capi.default_config(), n)
     rng = np.random.default_rng(0)
     t0 = time.time()
@@ -212,9 +247,9 @@ def run_bedbathing(args):
     reset_s = time.time() - t0
     stream = torch.cuda.ExternalStream(sim.stream_ptr())
     dev = torch.device('cuda')
-    act = (torch.rand((K + W, n, 7), device=dev) * 2 - 1) * args.action_scale
+    act = (torch.rand((K + W, n, 7), generator=torch.Generator(device=dev).manual_seed(0), device=dev) * 2 - 1) * args.action_scale
     obs = torch.zeros((n, 24), device=dev); rew = torch.zeros(n, device=dev); done = torch.zeros(n, device=dev); info = torch.zeros((n, 4), device=dev)
-    torch.cuda.synchronize()
+    device_mb = device_mb_since(free0)
     for i in range(W):
         sim.bathing_step_dev(act[i].data_ptr(), obs.data_ptr(), rew.data_ptr(), done.data_ptr(), info.data_ptr())
     torch.cuda.synchronize()
@@ -230,6 +265,8 @@ def run_bedbathing(args):
     torch.cuda.synchronize()
     clk = clocks.stop()
     ms = a.elapsed_time(b) / K
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {'obs': obs.cpu(), 'reward': rew.cpu(), 'done': done.cpu(), 'info': info.cpu()})
     cnt, it = sim.solver_stats()
     host_a = (np.random.default_rng(1).uniform(-1, 1, size=(K, n, 7)) * args.action_scale).astype(np.float32)
     sim.bathing_step_host(host_a[0])
@@ -241,7 +278,7 @@ def run_bedbathing(args):
     print(json.dumps({'metric': 'env-steps/sec BedBathingSawyer-v1 @batch%d' % n, 'value': n / ms * 1e3, 'unit': 'env-steps/s', 'n_gpus': 1, 'steps': K, 'warmup': W,
                       'ms_per_step': ms, 'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None, 'dtype': 'f32', 'data': 'synthetic',
                       'config': {'workload': 'BedBathingSawyer-v1, batch %d, fused step, wiping pad started pressed %.0f mm into the forearm, random actions x %.2f' % (n, args.press_mm, args.action_scale),
-                                 'global_batch': n, 'l2': 'not flushed (back-to-back steps)', 'reset_s': reset_s,
+                                 'global_batch': n, 'l2': 'not flushed (back-to-back steps)', 'reset_s': reset_s, 'device_memory_mb': device_mb,
                                  'ik_unresolved': int((ik_err >= 0.03).sum()),
                                  'contacts_per_env': {'mean': float(cnt.mean()), 'p99': float(np.percentile(cnt, 99)), 'max': int(cnt.max())},
                                  'envs_with_tool_force': float((force > 0).mean()), 'tool_force_mean_N': float(force[force > 0].mean()) if (force > 0).any() else 0.0,
@@ -251,7 +288,7 @@ def run_bedbathing(args):
 
 
 def run_dressing(args):
-    """BASELINE.json configs[3]: DressingPR2-v1 @ batch 2048 on one B200 (cloth-capsule contact path), fused step: device-timed
+    """BASELINE.json configs[3]: DressingPR2-v1 @ batch 2048 on one GPU (cloth-capsule contact path), fused step: device-timed
     value, host-buffer e2e, the roofline of k_cloth (the one HBM-shaped kernel of the repo: SURVEY.md 8(d), 190 KB of cloth
     state per env and substep) and the CPU oracle on a bounded sample."""
     import torch
@@ -288,6 +325,7 @@ def run_dressing(args):
                           'cpu_baseline': {'value': v, 'unit': 'env-steps/s', 'cores': cores, 'kind': 'port', 'sample': '%d envs x %d stepSimulation (%.1f s)' % (ne, steps, dt)},
                           'e2e': {'value': v, 'unit': 'env-steps/s', 'h2d_bytes_per_step': 0, 'd2h_bytes_per_step': 0}}))
         return
+    free0 = torch.cuda.mem_get_info()[0]
     sim = BatchSim(db.scene, cfg, n)
     t0 = time.time()
     smp = db.reset(sim, rng, attempts=args.toc_attempts, settle_steps=50)
@@ -295,9 +333,9 @@ def run_dressing(args):
     reset_s = time.time() - t0
     stream = torch.cuda.ExternalStream(sim.stream_ptr())
     dev = torch.device('cuda')
-    act = torch.rand((K + W, n, 7), device=dev) * 2 - 1
+    act = torch.rand((K + W, n, 7), generator=torch.Generator(device=dev).manual_seed(0), device=dev) * 2 - 1
     obs = torch.zeros((n, 24), device=dev); rew = torch.zeros(n, device=dev); done = torch.zeros(n, device=dev); info = torch.zeros((n, 4), device=dev)
-    torch.cuda.synchronize()
+    device_mb = device_mb_since(free0)
     for i in range(W):
         sim.dressing_step_dev(act[i].data_ptr(), obs.data_ptr(), rew.data_ptr(), done.data_ptr(), info.data_ptr())
     torch.cuda.synchronize()
@@ -314,6 +352,8 @@ def run_dressing(args):
     launches = sim.kernel_launches() - l0
     clk = clocks.stop()
     ms = a.elapsed_time(b) / K
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {'obs': obs.cpu(), 'reward': rew.cpu(), 'done': done.cpu(), 'info': info.cpu()})
     # per-kernel split in a separate pass (events around every launch, no graph)
     sim.profile_enable(True)
     for i in range(2):
@@ -348,7 +388,7 @@ def run_dressing(args):
                       'ms_per_step': ms, 'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None, 'dtype': 'f32', 'data': 'synthetic',
                       'config': {'workload': 'DressingPR2-v1, batch %d, fused step: 5 x (8 rigid substeps + 1 cloth launch), gown 3966 nodes / 11640 links, 5 position iterations, random actions' % n,
                                  'global_batch': n, 'l2': 'not flushed; the per-step working set (cloth state %d MB) exceeds L2' % (n * nn * 6 * 4 // 2 ** 20),
-                                 'reset_s': reset_s, 'toc_attempts': args.toc_attempts, 'goals_reached_mean': float(np.mean(db.goals_reached)), 'base_unresolved': int(db.unresolved),
+                                 'reset_s': reset_s, 'device_memory_mb': device_mb, 'toc_attempts': args.toc_attempts, 'goals_reached_mean': float(np.mean(db.goals_reached)), 'base_unresolved': int(db.unresolved),
                                  'cloth_contacts_per_env': {'mean': float(ccnt.mean()), 'p99': float(np.percentile(ccnt, 99)), 'max': int(ccnt.max())},
                                  'rigid_contacts_per_env': {'mean': float(rcnt.mean()), 'max': int(rcnt.max())},
                                  'envs_over_budget': over_steps, 'envs_over_budget_during_settle': over_settle, 'e2e_same_steps_as_value': True,
@@ -407,6 +447,7 @@ def main():
     ap.add_argument('--press-mm', type=float, default=5.0, help='bedbathing: start depth of the wiping pad in the forearm (SURVEY.md 8(d) C2: 5 mm)')
     ap.add_argument('--action-scale', type=float, default=0.2, help='bedbathing: scale of the random actions (small actions keep the pad on the skin)')
     ap.add_argument('--toc-attempts', type=int, default=10, help='dressing / bedbathing: random base poses ranked per reset (the reference uses 50)')
+    ap.add_argument('--dump-outputs', metavar='DIR', help='write the last timed step\'s obs / reward / done / info of rank 0\'s envs as DIR/<name>.npy (float32)')
     ap.add_argument('--sub-batches', type=int, default=int(os.environ.get('AG_SUB_BATCHES', '1')), help='independent sub-batches per GPU, each on its own stream')
     args = ap.parse_args()
     if args.workload == 'bedbathing':
@@ -436,6 +477,7 @@ def main():
     fb = FeedingBatch()
     cfg = capi.default_config()
     G = max(1, args.sub_batches)
+    free0 = torch.cuda.mem_get_info(local_rank)[0]
     sim = BatchSimGroup(fb.scene, cfg, n, groups=G, device=local_rank)
     # per-env seeds derive from the GLOBAL env id so results do not depend on the partition
     from assistive_gym_b200.sharding import sample_block, shard_range
@@ -462,7 +504,8 @@ def main():
     rew_db = [torch.zeros(n, device=dev) for _ in range(2)] if world > 1 else None
     rew_all = [torch.zeros(world * n, device=dev) for _ in range(2)] if world > 1 else None
     side = torch.cuda.Stream(device=dev) if world > 1 else None
-    flush = torch.empty(256 * 1024 * 1024 // 4, device=dev)      # 256 MiB > 126 MB L2
+    device_mb = device_mb_since(free0, dev)                       # before the L2-flush buffer, which is the bench's alone
+    flush = torch.empty(256 * 1024 * 1024 // 4, device=dev)      # 256 MiB, five times the H100's 50 MB L2
     torch.cuda.synchronize()
 
     def gather_reward(i, src):
@@ -519,6 +562,8 @@ def main():
     elapsed_ms = float(t.item())
     value = world * n * K / (elapsed_ms / 1000.0)
     rew_value_path = rew.detach().cpu().numpy().copy()        # reward of the last timed step (compared with the e2e path below)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {'obs': obs.cpu(), 'reward': rew_value_path, 'done': done.cpu(), 'info': info.cpu()})
     # the same K steps timed back to back (no flush, no per-step sync): how much the pipeline overlap is worth
     torch.cuda.synchronize()
     with torch.cuda.stream(stream):
@@ -603,7 +648,7 @@ def main():
                'data': 'synthetic',
                'config': {'workload': 'FeedingJaco-v1, batch %d per GPU, 5 substeps/step, 50 PGS iters (early exit 1e-7), random actions' % n,
                           'global_batch': world * n, 'parallelism': 'env-sharded x%d' % world,
-                          'l2': 'flushed between timed steps (256 MiB fill)', 'contact_budget': int(cfg.max_contacts),
+                          'l2': 'flushed between timed steps (256 MiB fill)', 'contact_budget': int(cfg.max_contacts), 'device_memory_mb': device_mb,
                           'envs_over_contact_budget': overflow,
                           'contacts_per_env': {'mean': float(ccount.mean()), 'p50': float(np.percentile(ccount, 50)), 'p99': float(np.percentile(ccount, 99)), 'max': int(ccount.max())},
                           'pgs_iters_per_env': {'mean': float(citers.mean()), 'p50': float(np.percentile(citers, 50)), 'p99': float(np.percentile(citers, 99)), 'max': int(citers.max())},

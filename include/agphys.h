@@ -1,8 +1,8 @@
-/* agphys.h — C ABI of the B200-native batched physics step for Assistive Gym.
+/* agphys.h — C ABI of the H100-native batched physics step for Assistive Gym.
  *
  * Drop-in boundary: the reference drives its physics through ~60 `pybullet` C-extension calls
  * (SURVEY.md §8(b)); every entry point below cites the reference call site(s) it replaces
- * (paths relative to /root/reference/assistive_gym/envs).  The host-side mirror
+ * (paths relative to the reference's assistive_gym/envs).  The host-side mirror
  * (`assistive_gym_b200/capi.py` + `assistive_gym_b200/sim.py`) binds these with ctypes; INTEGRATION.md shows the stub a
  * maintainer of the reference would add.
  *

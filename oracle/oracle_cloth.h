@@ -2,7 +2,7 @@
 // tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may use it.
 //
 // Follows, call by call, what `p.stepSimulation` does to the `btSoftBody` the reference creates with
-// p.loadCloth / p.clothParams (envs/dressing.py:146-154) -- Bullet's soft-body code is not under /root/reference
+// p.loadCloth / p.clothParams (envs/dressing.py:146-154) -- Bullet's soft-body code is not in the reference repository
 // (third-party: bullet3, Zackory fork, pinned by setup.py:21 only as "pybullet"), so this restates its published
 // algorithm as recalled (btSoftBody.cpp: predictMotion, addAeroForceToNode, ApplyClampedForce, solveConstraints,
 // PSolve_Anchors, PSolve_RContacts, PSolve_Links; btSoftBodyInternals.h: CollideSDF_RS::DoNode, checkContact).

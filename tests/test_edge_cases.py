@@ -1,5 +1,5 @@
 """Edge cases and size-independent properties of the batched step (host-compiled kernel bodies on CPU,
-the CUDA build on the B200): empty row streams, ragged batch sizes, batch-position invariance, state
+the CUDA build on the H100): empty row streams, ragged batch sizes, batch-position invariance, state
 round trips, contact-budget overflow, ABI error behaviour."""
 import numpy as np
 import pytest

@@ -1,7 +1,7 @@
 """Batched reset (SURVEY.md §8(f)1 / reference env.py:276-310): every env starts from a pose the reference would accept --
 IK converged and neither the arm nor the tool it holds intersects the person, the table or the wheelchair.  An env that
 starts in collision keeps 60-128 contacts for its whole episode and single-handedly sets the duration of the
-narrowphase and PGS kernels of the whole batch (profiles/README.md)."""
+narrowphase and PGS kernels of the whole batch."""
 import numpy as np
 
 from assistive_gym_b200 import capi

@@ -122,11 +122,11 @@ def test_assistive_gym_shim_resolves_reference_ids():
 
 
 def test_committed_bench_lines_follow_the_contract():
-    """The bench lines kept under profiles/ (written by bench.py on the GPU box) carry every key the measurement contract names."""
+    """The bench lines kept under profiles/ (written by bench.py on an H100) carry every key the measurement contract names."""
     import glob
     import json
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    files = sorted(glob.glob(os.path.join(root, 'profiles', 'r02[w-z]_bench*.json')))
+    files = sorted(glob.glob(os.path.join(root, 'profiles', 'h100_bench*.json')))
     assert files
     base = {'metric', 'value', 'unit', 'n_gpus', 'steps', 'warmup', 'ms_per_step', 'higher_is_better', 'scaling', 'vs_baseline', 'dtype', 'data', 'config', 'e2e'}
     for f in files:
