@@ -251,6 +251,7 @@ def load_library(path=None):
     lib.ag_get_solver_stats.argtypes = [vp, vp, vp]
     lib.ag_get_pgs_cycles.argtypes = [vp, vp]
     lib.ag_get_pgs_trips.argtypes = [vp, vp, vp]
+    lib.ag_get_pgs_occupancy.argtypes = [vp, vp, vp]
     lib.ag_profile_enable.argtypes = [vp, ci]
     lib.ag_profile_get.argtypes = [vp, ci, vp, ci, vp, vp]
     if path is None:
@@ -268,5 +269,5 @@ EXPORTED_SYMBOLS = [
     'ag_feeding_step_host', 'ag_feeding_step_host_begin', 'ag_feeding_step_host_end', 'ag_state_size', 'ag_state_get', 'ag_state_set', 'ag_kernel_launches',
     'ag_cloth_init', 'ag_cloth_set_state', 'ag_cloth_get_state', 'ag_cloth_set_anchor', 'ag_cloth_anchor_follow', 'ag_cloth_set_gravity',
     'ag_cloth_get_contacts', 'ag_cloth_device_state', 'ag_scratch_init', 'ag_scratch_step_dev', 'ag_scratch_step_host', 'ag_render', 'ag_set_body_gravity', 'ag_get_link_aabb', 'ag_dressing_init', 'ag_dressing_reset_episode', 'ag_dressing_set_tremor', 'ag_set_motor_force_scale', 'ag_dressing_step_dev', 'ag_dressing_step_host',
-    'ag_overflow_count', 'ag_get_solver_stats', 'ag_get_pgs_cycles', 'ag_get_pgs_trips', 'ag_profile_enable', 'ag_profile_get',
+    'ag_overflow_count', 'ag_get_solver_stats', 'ag_get_pgs_cycles', 'ag_get_pgs_trips', 'ag_get_pgs_occupancy', 'ag_profile_enable', 'ag_profile_get',
 ]

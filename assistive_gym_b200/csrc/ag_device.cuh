@@ -734,7 +734,7 @@ AG_HDN inline void dyn_body(int tid, const SimDev& S, const KP&) {
 
 // ------------------------------------------------------------------ K8: apply deltas, integrate
 // `dvf(i)`: solver delta of velocity entry i (dofs first, then 6 per free body); items are dealt to `stride` lanes
-// starting at `first` (the PGS kernel integrates with the 8 lanes of the env's group straight from shared memory,
+// starting at `first` (the PGS kernel integrates with the 4 lanes of the env's group straight from shared memory,
 // the stand-alone kernel with one lane from S.dv).
 template <class DV>
 AG_HD void integrate_env(int e, const SimDev& S, DV dvf, int first, int stride) {

@@ -8,30 +8,30 @@
 //
 // Design (round 2).  The Gauss-Seidel chain of one env is strictly sequential, so K7's speed is
 // the latency and the instruction count of one row update; round 1 ran it on ONE lane per env
-// (~450 cycles and ~115 warp instructions per row).  Now EIGHT lanes cooperate on an env and a warp
-// carries four envs in lock-step:
+// (~450 cycles and ~115 warp instructions per row).  Now FOUR lanes cooperate on an env and a warp
+// carries eight envs in lock-step:
 //   * the env's velocity-delta vector lives in shared memory in 8-float blocks (one block per free
-//     body, one or two per articulation); lane l of the env's lane group owns entries 8j + l, so a
-//     row's J.v is one FMA per lane per block plus a 3-level xor-shuffle reduction, and the update
-//     v += M^-1 J^T dlambda is one FMA per lane per block -- no cross-lane traffic through memory;
+//     body, one or two per articulation); lane l of the env's lane group owns entries 8j + 2l and
+//     8j + 2l + 1, so a row's J.v is two FMA chains per lane per block, one add and a 2-level
+//     xor-shuffle reduction -- the same summation tree as one lane per entry --, and the update
+//     v += M^-1 J^T dlambda is two FMAs per lane per block -- no cross-lane traffic through memory;
 //   * K6 writes the rows as RECORDS in one env-major stream (HBM/L2): a 64 B header (indices, rhs,
-//     1/diag, bounds) and up to four 128 B lane blocks, lane-major ([lane][J1 M1 J2 M2]), so a lane
-//     fetches its share of a block with ONE LDS.128;
+//     1/diag, bounds) and up to four 128 B lane blocks, entry-major ([entry][J1 M1 J2 M2]), so a lane
+//     fetches its share of a block with two LDS.128;
 //   * a record carries TWO rows that act on the same pair of bodies: two consecutive box rows
 //     (limit / motor / fixed-constraint / contact-normal) with their Gauss-Seidel coupling
 //     w21 = J2 M^-1 J1^T precomputed by K6 (row 2 sees row 1's update through one scalar FMA, which
 //     is algebraically the sequential sweep), or the two friction rows of a contact (solved jointly
 //     against the cone).  Both rows share the loads and the shuffle reduction;
-//   * the read-only stream is pulled from L2 by TMA bulk copies (cp.async.bulk + mbarrier
-//     complete_tx) into a two-deep ring of 2 KB chunks per env, issued by the lane group's first
-//     lane, the next chunk in flight while the current one is solved; the next record's header is
-//     loaded while the current record's reduction is in flight.
+//   * the read-only stream flows through a 4 KB ring per env: the first tile by a TMA bulk copy
+//     (cp.async.bulk + mbarrier complete_tx), then cp.async pieces right behind the consumer (see
+//     pgs_warp); the next record's header and lane blocks are loaded while the current record is solved.
 // Records never straddle a chunk (the packer pads).
 #pragma once
 #include "ag_device.cuh"
 
 #define RS_HDR 16             // header floats (64 B)
-#define RS_LB 32              // floats per lane block: 8 lanes x [J1 M1 J2 M2] (128 B)
+#define RS_LB 32              // floats per lane block: 8 entries x [J1 M1 J2 M2] (128 B)
 #define RS_UNIT 16            // record sizes / offsets are multiples of 16 floats
 #define RS_MAXREC (RS_HDR + 4 * RS_LB)
 // record modes
@@ -44,7 +44,7 @@ enum { RM_BOX = 0, RM_CONE = 1, RM_PAD = 2 };
 //   [4] lin                                              RM_CONE: impulse of the contact's normal row
 //   [5] w21   [6] mu   [7] -
 //   [8..11] rhs1 dinv1 lo1 hi1   [12..15] rhs2 dinv2 lo2 hi2     (RM_CONE ignores lo/hi)
-// Lane block k, lane l: [J1 M1 J2 M2] of velocity entry slot_k + l.  Unused slots point at the env's null block
+// Lane block k, quad i: [J1 M1 J2 M2] of velocity entry slot_k + i.  Unused slots point at the env's null block
 // (8 zeros at the end of the velocity vector), an absent second row has li2 = the dummy impulse and all-zero data.
 
 struct alignas(16) v4 { float x, y, z, w; };
@@ -59,9 +59,14 @@ AG_HD int rs_nv(const SimDev& S) { return (S.NDp + 8 * S.nf + 8 + 31) & ~31; }
 // impulses: [3 ND dof rows][ngr fixed-constraint rows][3 per contact][dummy]
 AG_HD int rs_dummy(const SimDev& S) { return 3 * S.ND + S.ngr + 3 * S.maxc; }
 AG_HD int rs_nlam(const SimDev& S) { return (3 * S.ND + S.ngr + 3 * S.maxc + 1 + 31) & ~31; }
-// shared memory of a K7 CTA (four envs): per env velocity deltas, impulses, 32 zeros, a null record, the 4 KB stream ring
+// shared memory of a K7 CTA (RS_CTA_ENVS envs): 4 KB alignment slack, per env the 4 KB stream ring, per env velocity
+// deltas and impulses (stride rs_env_stride), one 8-byte mbarrier per env
+#define RS_CTA_ENVS 8
 AG_HD int rs_env_floats(const SimDev& S) { return rs_nv(S) + rs_nlam(S) + 64 + 1024; }      // (host emulation layout)
-AG_HD int rs_cta_floats(const SimDev& S) { return 1024 + 4 * 1024 + 4 * (rs_nv(S) + rs_nlam(S)); }
+// +8 floats: consecutive envs' vectors start 32 B apart modulo 128 B, so the eight lane groups' 32-byte velocity accesses
+// to the same entries fall into different banks
+AG_HD int rs_env_stride(const SimDev& S) { return rs_nv(S) + rs_nlam(S) + 8; }
+AG_HD int rs_cta_floats(const SimDev& S) { return 1024 + RS_CTA_ENVS * (1024 + rs_env_stride(S)) + 2 * RS_CTA_ENVS; }
 
 // ------------------------------------------------------------------ K6: constraint rows
 // side reference encoding: (idx << 2) | kind, kind: 0 static, 1 free body (idx = f), 2 articulated (idx = dyn link)
@@ -591,7 +596,7 @@ AG_HDN inline void crows_body(int tid, const SimDev& S, const KP&) {
 
 // ------------------------------------------------------------------ K6c: heaviest-first env order for K7
 // The PGS chain of an env is sequential and its length varies 10x between envs (iterations used x
-// rows); the four envs of a K7 warp run in lock-step, so envs of similar weight share a warp and the
+// rows); the eight envs of a K7 warp run in lock-step, so envs of similar weight share a warp and the
 // heaviest warps are issued first.  Work is predicted from this substep's stream length and the
 // previous substep's iteration count.  One CTA: 64-bucket counting sort in shared memory.
 AG_HD int pgs_work_bucket(const SimDev& S, int e) {
@@ -604,7 +609,7 @@ AG_HD int pgs_work_bucket(const SimDev& S, int e) {
 // ------------------------------------------------------------------ K7: PGS over the row stream
 // The two rows of a record, given J1.v and J2.v (p1, p2) and the current impulses: new impulses and their changes.
 struct RsSol { float s1, s2, d1, d2; };
-// Branch-free on the device: the four envs of a warp are at records of different modes, and a divergent branch in
+// Branch-free on the device: the eight envs of a warp are at records of different modes, and a divergent branch in
 // front of the warp-wide shuffles costs more than the few selects.  Everything that does not depend on p1 / p2 (the
 // reduced J.v) is computed ahead of them: the dependent chain is fma, max, min, sub, fma, fma, max, min, sub.
 // `dead`: the env has finished; the record is consumed without effect (bounds collapse onto the current impulses).
@@ -673,12 +678,14 @@ __device__ __forceinline__ void rs_wait(rs_addr bar, unsigned parity) {
                  : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
   } while (!ok);
 }
-__device__ __forceinline__ float rs_sum8(float x) {            // sum over the 8 lanes of a lane group (bitwise equal on all 8)
-  x += __shfl_xor_sync(0xffffffffu, x, 1);
-  x += __shfl_xor_sync(0xffffffffu, x, 2);
-  x += __shfl_xor_sync(0xffffffffu, x, 4);
-  return x;
+// The loop's per-entry arithmetic with its rounding pinned (explicit fma / mul / add, no contraction left to the
+// compiler), so that the lane partition can change without changing a bit of the result:
+//   J.v over the four blocks of one velocity entry: (j0 x0 + j1 x1) + (j2 x2 + j3 x3);
+__device__ __forceinline__ float rs_jv(float j0, float x0, float j1, float x1, float j2, float x2, float j3, float x3) {
+  return __fadd_rn(__fmaf_rn(j0, x0, __fmul_rn(j1, x1)), __fmaf_rn(j2, x2, __fmul_rn(j3, x3)));
 }
+//   the velocity update of one entry: x + m1 d1 + m2 d2.
+__device__ __forceinline__ float rs_dv(float x, float m1, float d1, float m2, float d2) { return __fmaf_rn(m2, d2, __fmaf_rn(m1, d1, x)); }
 struct RsHdr { v4 a, b, c, d; };
 // 16-byte asynchronous copy global -> shared by the executing lane (LDGSTS), predicated, with a compile-time byte offset
 template <int OFF> __device__ __forceinline__ void rs_cp16(rs_addr dst, const void* src, bool on) {
@@ -692,16 +699,17 @@ __device__ __forceinline__ float rs_lds(rs_addr a) { float r; asm volatile("ld.s
 template <int OFF> __device__ __forceinline__ v4 rs_lds4(rs_addr a) {
   v4 r; asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4+%5];" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "r"(a), "n"(OFF)); return r;
 }
-__device__ __forceinline__ float rs_lds_if(rs_addr a, bool on) {            // 0 if not `on`
-  float r; asm volatile("{ .reg .pred p; setp.ne.b32 p, %2, 0; mov.f32 %0, 0f00000000; @p ld.shared.f32 %0, [%1]; }" : "=f"(r) : "r"(a), "r"((int)on)); return r;
+__device__ __forceinline__ float2 rs_lds2_if(rs_addr a, bool on) {         // zeros if not `on`
+  float2 r; asm volatile("{ .reg .pred p; setp.ne.b32 p, %3, 0; mov.f32 %0, 0f00000000; mov.f32 %1, 0f00000000; @p ld.shared.v2.f32 {%0, %1}, [%2]; }"
+                         : "=f"(r.x), "=f"(r.y) : "r"(a), "r"((int)on)); return r;
 }
-__device__ __forceinline__ v4 rs_lds4_if(rs_addr a, bool on) {              // zeros if not `on`
+template <int OFF> __device__ __forceinline__ v4 rs_lds4_if(rs_addr a, bool on) {   // zeros if not `on`
   v4 r; asm volatile("{ .reg .pred p; setp.ne.b32 p, %5, 0; mov.f32 %0, 0f00000000; mov.f32 %1, 0f00000000; mov.f32 %2, 0f00000000; mov.f32 %3, 0f00000000;\n"
-                     "  @p ld.shared.v4.f32 {%0, %1, %2, %3}, [%4]; }" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "r"(a), "r"((int)on)); return r;
+                     "  @p ld.shared.v4.f32 {%0, %1, %2, %3}, [%4+%6]; }" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "r"(a), "r"((int)on), "n"(OFF)); return r;
 }
 __device__ __forceinline__ void rs_sts(rs_addr a, float x) { asm volatile("st.shared.f32 [%0], %1;" :: "r"(a), "f"(x)); }
-__device__ __forceinline__ void rs_sts_if(rs_addr a, float x, bool on) {
-  asm volatile("{ .reg .pred p; setp.ne.b32 p, %2, 0; @p st.shared.f32 [%0], %1; }" :: "r"(a), "f"(x), "r"((int)on));
+__device__ __forceinline__ void rs_sts2_if(rs_addr a, float x, float y, bool on) {
+  asm volatile("{ .reg .pred p; setp.ne.b32 p, %3, 0; @p st.shared.v2.f32 [%0], {%1, %2}; }" :: "r"(a), "f"(x), "f"(y), "r"((int)on));
 }
 __device__ __forceinline__ void rs_sts4_if(rs_addr a, v4 x, bool on) {
   asm volatile("{ .reg .pred p; setp.ne.b32 p, %5, 0; @p st.shared.v4.f32 [%0], {%1, %2, %3, %4}; }" :: "r"(a), "f"(x.x), "f"(x.y), "f"(x.z), "f"(x.w), "r"((int)on));
@@ -711,19 +719,19 @@ __device__ __forceinline__ rs_addr rs_wrap(rs_addr ring, int byte) {        // r
 }
 
 #define RS_RING 1024          // floats of an env's stream ring (4 KB, 4 KB aligned)
-#define RS_PIECE 32           // floats per refill piece: 8 lanes x 16 B
+#define RS_PIECE 32           // floats per refill piece: 4 lanes x 32 B
 #define RS_KPF 6              // refill pieces per record consumed (192 floats > the largest record: the ring stays full)
 #define RS_WAITG 3            // cp.async groups (= records) that may still be in flight
 
 // One record of one env group.  (H, Q): header and lane blocks of the record solved now (loaded one trip earlier);
-// (Hn, Qn): filled with the next record's.  See pgs_warp.
-#define RS_TRIP(H, Q0_, Q1_, Q2_, Q3_, Hn, Qn0_, Qn1_, Qn2_, Qn3_)                                                        \
+// (Hn, Qn): filled with the next record's.  Q[2k], Q[2k + 1]: quads 2l and 2l + 1 of lane block k.  See pgs_warp.
+#define RS_TRIP(H, Q, Hn, Qn)                                                                                             \
   {                                                                                                                       \
     const int meta = f2i_bits(H.a.x), w1 = f2i_bits(H.a.y), w2 = f2i_bits(H.a.z), w3 = f2i_bits(H.a.w);                   \
     const int nv = meta & 7, mode = (meta >> 4) & 3;                                                                      \
     const rs_addr a0 = vbl + (w1 & 0xffff), a1 = vbl + ((unsigned)w1 >> 16), a2 = vbl + (w2 & 0xffff), a3 = vbl + ((unsigned)w2 >> 16); \
     const rs_addr l1 = vb + (w3 & 0xffff), l2 = vb + ((unsigned)w3 >> 16), ln = vb + f2i_bits(H.b.x);                     \
-    const float x0 = rs_lds_if(a0, nv > 0), x1 = rs_lds_if(a1, nv > 1), x2 = rs_lds_if(a2, nv > 2), x3 = rs_lds_if(a3, nv > 3); \
+    const float2 x0 = rs_lds2_if(a0, nv > 0), x1 = rs_lds2_if(a1, nv > 1), x2 = rs_lds2_if(a2, nv > 2), x3 = rs_lds2_if(a3, nv > 3); \
     const float lam1 = rs_lds(l1), lam2 = rs_lds(l2), lamn = rs_lds(ln);                                                  \
     const int adv = active ? (int)((unsigned)meta >> 8) : 0;                                                              \
     const int nb = cb + adv;                                                                                              \
@@ -734,78 +742,87 @@ __device__ __forceinline__ rs_addr rs_wrap(rs_addr ring, int byte) {        // r
     __syncwarp();                               /* pieces copied by the other lanes of the group */                       \
     const rs_addr ha = rs_wrap(ring_s, nb);                                                                               \
     Hn.a = rs_lds4<0>(ha); Hn.b = rs_lds4<16>(ha); Hn.c = rs_lds4<32>(ha); Hn.d = rs_lds4<48>(ha);                         \
-    float p1 = (Q0_.x * x0 + Q1_.x * x1) + (Q2_.x * x2 + Q3_.x * x3);                                                     \
-    float p2 = (Q0_.z * x0 + Q1_.z * x1) + (Q2_.z * x2 + Q3_.z * x3);                                                     \
+    /* the partial sums of entries 2l and 2l + 1, added in a register: J.v is reduced over the same tree as with one */  \
+    /* lane per entry (pairs, then xor 1 = pairs of pairs, then xor 2)                                                */  \
+    float p1 = rs_jv(Q[0].x, x0.x, Q[2].x, x1.x, Q[4].x, x2.x, Q[6].x, x3.x) + rs_jv(Q[1].x, x0.y, Q[3].x, x1.y, Q[5].x, x2.y, Q[7].x, x3.y); \
+    float p2 = rs_jv(Q[0].z, x0.x, Q[2].z, x1.x, Q[4].z, x2.x, Q[6].z, x3.x) + rs_jv(Q[1].z, x0.y, Q[3].z, x1.y, Q[5].z, x2.y, Q[7].z, x3.y); \
     p1 += __shfl_xor_sync(0xffffffffu, p1, 1); p2 += __shfl_xor_sync(0xffffffffu, p2, 1);                                 \
-    p1 += __shfl_xor_sync(0xffffffffu, p1, 2); p2 += __shfl_xor_sync(0xffffffffu, p2, 2);                                 \
     /* refill: everything in front of the next record is consumed; up to RS_KPF pieces of 128 B right behind the */      \
     /* requests so far, not across the end of the ring or of the sweep (the next trip goes on from there)         */      \
     {                                                                                                                     \
       int n = min(min((nb + 4096 - pbyte) >> 7, (4096 - (pbyte & 4095)) >> 7), min((totalB - ppos) >> 7, RS_KPF));       \
       n = active ? n : 0;                                                                                                 \
-      const rs_addr dst = rs_wrap(ring_s, pbyte) + 16 * l;                                                                \
+      const rs_addr dst = rs_wrap(ring_s, pbyte) + 32 * l;                                                                \
       const char* src = rsl + ppos;                                                                                       \
-      rs_cp16<0>(dst, src, n > 0); rs_cp16<128>(dst, src, n > 1); rs_cp16<256>(dst, src, n > 2);                          \
-      rs_cp16<384>(dst, src, n > 3); rs_cp16<512>(dst, src, n > 4); rs_cp16<640>(dst, src, n > 5);                        \
+      rs_cp16<0>(dst, src, n > 0); rs_cp16<16>(dst, src, n > 0); rs_cp16<128>(dst, src, n > 1); rs_cp16<144>(dst, src, n > 1); \
+      rs_cp16<256>(dst, src, n > 2); rs_cp16<272>(dst, src, n > 2); rs_cp16<384>(dst, src, n > 3); rs_cp16<400>(dst, src, n > 3); \
+      rs_cp16<512>(dst, src, n > 4); rs_cp16<528>(dst, src, n > 4); rs_cp16<640>(dst, src, n > 5); rs_cp16<656>(dst, src, n > 5); \
       rs_cp_commit();                                                                                                     \
       pbyte += n << 7; ppos += n << 7;                                                                                    \
       ppos = ppos == totalB ? 0 : ppos;                                                                                   \
     }                                                                                                                     \
-    p1 += __shfl_xor_sync(0xffffffffu, p1, 4); p2 += __shfl_xor_sync(0xffffffffu, p2, 4);                                 \
+    p1 += __shfl_xor_sync(0xffffffffu, p1, 2); p2 += __shfl_xor_sync(0xffffffffu, p2, 2);                                 \
     const RsSol r = rs_solve2(mode, cone_cfg, !active, p1, p2, lam1, lam2, lamn, H.c, H.d, H.b.y, H.b.z);                 \
     rs_sts(l1, r.s1); rs_sts(l2, r.s2);                                                                                   \
-    rs_sts_if(a0, x0 + Q0_.y * r.d1 + Q0_.w * r.d2, nv > 0);                                                              \
-    rs_sts_if(a1, x1 + Q1_.y * r.d1 + Q1_.w * r.d2, nv > 1);                                                              \
-    rs_sts_if(a2, x2 + Q2_.y * r.d1 + Q2_.w * r.d2, nv > 2);                                                              \
-    rs_sts_if(a3, x3 + Q3_.y * r.d1 + Q3_.w * r.d2, nv > 3);                                                              \
+    rs_sts2_if(a0, rs_dv(x0.x, Q[0].y, r.d1, Q[0].w, r.d2), rs_dv(x0.y, Q[1].y, r.d1, Q[1].w, r.d2), nv > 0);             \
+    rs_sts2_if(a1, rs_dv(x1.x, Q[2].y, r.d1, Q[2].w, r.d2), rs_dv(x1.y, Q[3].y, r.d1, Q[3].w, r.d2), nv > 1);             \
+    rs_sts2_if(a2, rs_dv(x2.x, Q[4].y, r.d1, Q[4].w, r.d2), rs_dv(x2.y, Q[5].y, r.d1, Q[5].w, r.d2), nv > 2);             \
+    rs_sts2_if(a3, rs_dv(x3.x, Q[6].y, r.d1, Q[6].w, r.d2), rs_dv(x3.y, Q[7].y, r.d1, Q[7].w, r.d2), nv > 3);             \
     resid = fmaxf(resid, fmaxf(r.d1 * r.d1, r.d2 * r.d2));                                                                \
     it += at_end ? 1 : 0;                                                                                                 \
     const bool stop = at_end && ((thr > 0.f && resid <= thr) || it >= iters);                                             \
     resid = at_end ? 0.f : resid;                                                                                         \
     /* a finished env parks: a null record (size 0) goes where its next record would have been read */                   \
-    rs_sts4_if(ha + 16 * l, nullq, stop && l < 4);                                                                        \
+    rs_sts4_if(ha + 16 * l, nullq, stop);                                                                                 \
     active = active && !stop;                                                                                             \
     cb = nb;                                                                                                              \
-    /* lane blocks of the next record, last: its header has long arrived, so only its nv blocks are fetched */           \
+    /* lane blocks of the next record, last: its header has long arrived, so only its nv blocks are fetched; a lane's */ \
+    /* two quads of a block are adjacent and never straddle the end of the ring                                        */ \
     {                                                                                                                     \
       const int nvn = f2i_bits(Hn.a.x) & 7;                                                                               \
       const int bl = nb + cl;                                                                                             \
-      Qn0_ = rs_lds4_if(rs_wrap(ring_s, bl), nvn > 0); Qn1_ = rs_lds4_if(rs_wrap(ring_s, bl + 128), nvn > 1);             \
-      Qn2_ = rs_lds4_if(rs_wrap(ring_s, bl + 256), nvn > 2); Qn3_ = rs_lds4_if(rs_wrap(ring_s, bl + 384), nvn > 3);       \
+      const rs_addr q0 = rs_wrap(ring_s, bl), q1 = rs_wrap(ring_s, bl + 128), q2 = rs_wrap(ring_s, bl + 256), q3 = rs_wrap(ring_s, bl + 384); \
+      Qn[0] = rs_lds4_if<0>(q0, nvn > 0); Qn[1] = rs_lds4_if<16>(q0, nvn > 0);                                            \
+      Qn[2] = rs_lds4_if<0>(q1, nvn > 1); Qn[3] = rs_lds4_if<16>(q1, nvn > 1);                                            \
+      Qn[4] = rs_lds4_if<0>(q2, nvn > 2); Qn[5] = rs_lds4_if<16>(q2, nvn > 2);                                            \
+      Qn[6] = rs_lds4_if<0>(q3, nvn > 3); Qn[7] = rs_lds4_if<16>(q3, nvn > 3);                                            \
     }                                                                                                                     \
   }
 
-// One warp = four envs (lane group g = lane / 8), lock-step.  Shared memory: per env a 4 KB ring (4 KB aligned) through
-// which the env's row stream flows once per sweep, then per env velocity deltas and impulses:
+// One warp = eight envs (lane group g = lane / 4, lane l = lane % 4 of the group), lock-step.  Lane l owns entries 2l
+// and 2l + 1 of every 8-entry velocity block (one LDS.64 / STS.64 per block) and quads 2l and 2l + 1 of every lane
+// block (two LDS.128).  Shared memory: per env a 4 KB ring (4 KB aligned) through which the env's row stream flows
+// once per sweep, then per env velocity deltas and impulses:
 //   * the ring is filled by one TMA bulk copy per env (mbarrier complete_tx); a stream shorter than the ring wraps
 //     inside it and is staged by cp.async pieces instead,
-//   * from then on every lane copies 16 B pieces with cp.async right behind the consumer (up to RS_KPF pieces of 128 B
-//     per record and env), so the refill is SIMT-uniform -- no elected lane, no spin loop -- and a record is consumed
-//     RS_WAITG + 1 records after its bytes were requested (cp.async.wait_group).
-// The stream stays in HBM / L2; ~6.5 KB of shared memory per env keep every env of the batch resident at once.
+//   * from then on every lane copies its 32 B of each 128 B piece with two 16 B cp.async right behind the consumer (up
+//     to RS_KPF pieces per record and env), so the refill is SIMT-uniform -- no elected lane, no spin loop -- and a
+//     record is consumed RS_WAITG + 1 records after its bytes were requested (cp.async.wait_group).  Which bytes are
+//     requested when does not depend on how the lanes split a piece: tests/test_ring_protocol.py models the schedule.
+// The stream stays in HBM / L2; ~6.9 KB of shared memory per env keep every env of a 4096-env batch resident at once.
 // There is NO lane-dependent branch in front of the loop's shuffles: a diverged warp executes them on a collective slow
 // path that costs thousands of cycles per record (measured), so everything is selects and predicated instructions.
 __device__ __forceinline__ void pgs_warp(const SimDev& S, float* sm, int, int warp_slot0) {
-  const int lane = threadIdx.x & 31, g = lane >> 3, l = lane & 7;
+  const int lane = threadIdx.x & 31, g = lane >> 2, l = lane & 3;
   const int N = S.N;
   const int slot = warp_slot0 + g;
   const bool valid = slot < N;
   const int e = valid ? S.pgs_order[slot] : 0;
-  const int NV = rs_nv(S), NL = rs_nlam(S), EF = NV + NL;
+  const int NV = rs_nv(S), NL = rs_nlam(S), EF = NV + NL, ES = rs_env_stride(S);
   const rs_addr sm_s = rs_smem_addr(sm);
   const rs_addr ring0 = (sm_s + 4095u) & ~4095u;                    // the CTA asked for 4 KB of slack
   const rs_addr ring_s = ring0 + 4096u * g;
-  float* v = (float*)((char*)sm + (ring0 - sm_s) + 4 * 4096) + (size_t)g * EF;
-  const rs_addr vb = rs_smem_addr(v), vbl = vb + 4 * l;
-  const rs_addr bar = rs_smem_addr(v - (size_t)g * EF + (size_t)4 * EF) + 8 * g;
+  float* v = (float*)((char*)sm + (ring0 - sm_s) + RS_CTA_ENVS * 4096) + (size_t)g * ES;
+  const rs_addr vb = rs_smem_addr(v), vbl = vb + 8 * l;
+  const rs_addr bar = rs_smem_addr(v - (size_t)g * ES + (size_t)RS_CTA_ENVS * ES) + 8 * g;
   const long long t_begin = clock64();
-  for (int i = l; i < EF; i += 8) v[i] = 0.f;
+  for (int i = l; i < EF; i += 4) v[i] = 0.f;
   const float* rs = S.rs_data + (size_t)e * S.rs_cap;
-  const char* rsl = (const char*)(rs + 4 * l);
+  const char* rsl = (const char*)(rs + 8 * l);
   const int total = valid ? S.rs_nfloats[e] : 0;     // a multiple of RS_PIECE (K6a pads)
   const int totalB = total > 0 ? total * 4 : 128;
-  v4 nullq;                                          // lane l < 4: quad l of a null record's header
-  nullq.x = rs_null_word(S, 4 * (l & 3)); nullq.y = rs_null_word(S, 4 * (l & 3) + 1); nullq.z = rs_null_word(S, 4 * (l & 3) + 2); nullq.w = rs_null_word(S, 4 * (l & 3) + 3);
+  v4 nullq;                                          // quad l of a null record's header
+  nullq.x = rs_null_word(S, 4 * l); nullq.y = rs_null_word(S, 4 * l + 1); nullq.z = rs_null_word(S, 4 * l + 2); nullq.w = rs_null_word(S, 4 * l + 3);
   // ---- fill the ring (all of it: the stream repeats every sweep).  A stream of at least a ring: ONE TMA bulk copy;
   // a shorter one wraps inside the ring: 128 B pieces by cp.async; an env without rows: zeros and a null record.
   const bool big = total >= RS_RING;
@@ -817,26 +834,36 @@ __device__ __forceinline__ void pgs_warp(const SimDev& S, float* sm, int, int wa
     int pp = 0;
     v4 z; z.x = z.y = z.z = z.w = 0.f;
     for (int j = 0; j < RS_RING / RS_PIECE; j++) {
-      rs_cp16<0>(ring_s + 128 * j + 16 * l, rsl + pp, !big && total > 0);
-      rs_sts4_if(ring_s + 128 * j + 16 * l, z, total == 0);
+      rs_cp16<0>(ring_s + 128 * j + 32 * l, rsl + pp, !big && total > 0);
+      rs_cp16<16>(ring_s + 128 * j + 32 * l, rsl + pp, !big && total > 0);
+      rs_sts4_if(ring_s + 128 * j + 32 * l, z, total == 0);
+      rs_sts4_if(ring_s + 128 * j + 32 * l + 16, z, total == 0);
       pp += 128; pp = pp >= totalB ? 0 : pp;
     }
     rs_cp_commit();
     rs_cp_wait<0>();
     __syncwarp();
-    rs_sts4_if(ring_s + 16 * l, nullq, total == 0 && l < 4);
+    rs_sts4_if(ring_s + 16 * l, nullq, total == 0);
   }
   int ppos = (RS_RING * 4) % totalB, pbyte = RS_RING * 4;
   { bool ok; do { ok = big ? rs_try_wait(bar, 0) : true; } while (!__all_sync(0xffffffffu, ok)); }   // warp-uniform loop
   __syncwarp();
   bool active = total > 0 && S.iters > 0;
   int it = 0, cb = 0, left = totalB;
-  const int cl = 64 + 16 * l;
+  const int cl = 64 + 32 * l;
   RsHdr HA, HB;
-  v4 QA0, QA1, QA2, QA3, QB0, QB1, QB2, QB3;
+  v4 QA[8], QB[8];
   HA.a = rs_lds4<0>(ring_s); HA.b = rs_lds4<16>(ring_s); HA.c = rs_lds4<32>(ring_s); HA.d = rs_lds4<48>(ring_s);
-  { const int nv0 = f2i_bits(HA.a.x) & 7; QA0 = rs_lds4_if(ring_s + cl, nv0 > 0); QA1 = rs_lds4_if(ring_s + cl + 128, nv0 > 1); QA2 = rs_lds4_if(ring_s + cl + 256, nv0 > 2); QA3 = rs_lds4_if(ring_s + cl + 384, nv0 > 3); }
-  HB = HA; QB0 = QA0; QB1 = QA1; QB2 = QA2; QB3 = QA3;
+  {
+    const int nv0 = f2i_bits(HA.a.x) & 7;
+    QA[0] = rs_lds4_if<0>(ring_s + cl, nv0 > 0); QA[1] = rs_lds4_if<16>(ring_s + cl, nv0 > 0);
+    QA[2] = rs_lds4_if<128>(ring_s + cl, nv0 > 1); QA[3] = rs_lds4_if<144>(ring_s + cl, nv0 > 1);
+    QA[4] = rs_lds4_if<256>(ring_s + cl, nv0 > 2); QA[5] = rs_lds4_if<272>(ring_s + cl, nv0 > 2);
+    QA[6] = rs_lds4_if<384>(ring_s + cl, nv0 > 3); QA[7] = rs_lds4_if<400>(ring_s + cl, nv0 > 3);
+  }
+  HB = HA;
+#pragma unroll
+  for (int k = 0; k < 8; k++) QB[k] = QA[k];
   float resid = 0.f;
   const bool cone_cfg = S.cone != 0;
   const float thr = S.resid_thr;
@@ -847,23 +874,23 @@ __device__ __forceinline__ void pgs_warp(const SimDev& S, float* sm, int, int wa
   // The loop is software pipelined -- record t's header and lane blocks were loaded during record t-1 -- and unrolled
   // by two with the register sets swapped; the loop condition votes on the flag of two trips before (idle trips at the
   // end), so neither a load nor the vote sits on the dependent chain
-  //   LDS v -> fma -> 3 x (shfl, add) -> solve -> fma -> STS v.
+  //   LDS v -> fma -> add -> 2 x (shfl, add) -> solve -> fma -> STS v.
   while (__any_sync(0xffffffffu, act_lag) && --guard > 0) {
     act_lag = active;
-    RS_TRIP(HA, QA0, QA1, QA2, QA3, HB, QB0, QB1, QB2, QB3)
-    RS_TRIP(HB, QB0, QB1, QB2, QB3, HA, QA0, QA1, QA2, QA3)
+    RS_TRIP(HA, QA, HB, QB)
+    RS_TRIP(HB, QB, HA, QA)
   }
   rs_cp_wait<0>();
   __syncwarp();
   if (!valid) return;
-  // ---- write back and integrate (8 lanes per env): impulses for the read-back calls, then K8 straight from shared memory
+  // ---- write back and integrate (4 lanes per env): impulses for the read-back calls, then K8 straight from shared memory
   float* lam = v + NV;
   if (l == 0) { S.iters_used[e] = it; S.pgs_cycles[e] = (int)(clock64() - t_begin); S.pgs_trips[e] = 2 * (guard0 - guard); }
   const int ND = S.ND;
-  for (int r = l; r < S.ngr; r += 8) S.gr_lam[(size_t)r * N + e] = lam[3 * ND + r];
+  for (int r = l; r < S.ngr; r += 4) S.gr_lam[(size_t)r * N + e] = lam[3 * ND + r];
   int cnt = S.c_count[e]; if (cnt > S.maxc) cnt = S.maxc;
-  for (int i = l; i < 3 * cnt; i += 8) { int s = i / 3, c = i - 3 * s; cf_st(S.s_data, s, CF_LAM_N + c, N, e, lam[3 * ND + S.ngr + i]); }
-  for (int d = l; d < ND; d += 8) {
+  for (int i = l; i < 3 * cnt; i += 4) { int s = i / 3, c = i - 3 * s; cf_st(S.s_data, s, CF_LAM_N + c, N, e, lam[3 * ND + S.ngr + i]); }
+  for (int d = l; d < ND; d += 4) {
     int k = AG_LDG(S.dl_link + d);
     if (S.body_mode[(size_t)AG_LDG(S.link_body + k) * N + e] == 1) st1(S.motor_applied, k, N, e, lam[2 * ND + d] / S.dt);
   }
@@ -873,13 +900,14 @@ __device__ __forceinline__ void pgs_warp(const SimDev& S, float* sm, int, int wa
     if (i >= S->ND) { int f = (i - S->ND) / 6, c = (i - S->ND) - 6 * f; return v[S->NDp + 8 * f + c]; }
     int a = AG_LDG(S->dl_art + i); return v[AG_LDG(S->art_voff + a) + (i - AG_LDG(S->art_dl0 + a))];
   } } dvs; dvs.v = v; dvs.S = &S;
-  integrate_env(e, S, dvs, l, 8);
+  integrate_env(e, S, dvs, l, 4);
 }
 #endif
 
 // Host restatement of the DEVICE loop of K7 for one env (tests only): the same ring indexing, refill schedule, software
-// pipelining, finished-env parking, "blocks beyond nv are read but multiply zeros" and lane partition, with the
-// asynchronous copies done synchronously.  `sm`: rs_env_floats floats.
+// pipelining, finished-env parking and "blocks beyond nv are read but multiply zeros", with the asynchronous copies
+// done synchronously.  It works entry by entry; how the device deals the entries to lanes (four lanes, two entries
+// each) changes which lane computes what, not the byte schedule or the record order.  `sm`: rs_env_floats floats.
 AG_HDN inline void pgs_env_emul(int slot, const SimDev& S, float* sm) {
   const int RING = 1024, KPF = 6;
   const int e = S.pgs_order[slot];

@@ -61,13 +61,13 @@ AG_KERNEL(k_sort, sort_body)
 AG_KERNEL(k_dyn, dyn_body)
 AG_KERNEL(k_rows, rows_body)
 AG_KERNEL(k_crows, crows_body)
-// k_pgs: one warp per CTA = four envs, eight lanes each; per-env shared memory = velocity deltas + impulses +
-// a two-deep ring of 2 KB row-stream chunks filled by TMA bulk copies (see ag_solver.cuh).
+// k_pgs: one warp per CTA = RS_CTA_ENVS (8) envs, four lanes each; per-env shared memory = velocity deltas + impulses +
+// a 4 KB row-stream ring (TMA bulk copy for the first tile, cp.async refill; see ag_solver.cuh).
 // k_order: heaviest-first env order for k_pgs (64-bucket counting sort, one CTA).
 #ifndef AG_CPU_EMU
 __global__ void __launch_bounds__(32) k_pgs(SimDev S, KP p) {
   extern __shared__ __align__(128) float pgs_smem[];
-  pgs_warp(S, pgs_smem, p.i0, blockIdx.x * 4);
+  pgs_warp(S, pgs_smem, p.i0, blockIdx.x * RS_CTA_ENVS);
 }
 __global__ void __launch_bounds__(1024) k_order(SimDev S, KP) {
   __shared__ int hist[64];
@@ -518,7 +518,7 @@ AgSim* ag_create(const AgSceneDesc* d, const AgConfig* cfg, int n_envs, int devi
 #ifndef AG_CPU_EMU
   {
     { const char* gg = getenv("AG_GRAPH"); if (gg && atoi(gg) == 0) s->use_graph = false; }
-    size_t smem = (size_t)rs_cta_floats(S) * sizeof(float) + 32;
+    size_t smem = (size_t)rs_cta_floats(S) * sizeof(float);
     if (smem > 227 * 1024) { g_err = "PGS shared-memory footprint exceeds 227 KB per CTA: lower max_contacts"; ag_destroy(s); return nullptr; }
     if (cudaFuncSetAttribute(k_pgs, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { g_err = "cudaFuncSetAttribute(k_pgs) failed"; ag_destroy(s); return nullptr; }
   }
@@ -776,10 +776,10 @@ static void substep(AgSim* s) {
     k_order<<<1, 1024, 0, s->stream>>>(S, z);
     if (ps >= 0) prof_mark(s, ps, false);
     KP kp = z; kp.n = N;
-    size_t smem = (size_t)rs_cta_floats(S) * sizeof(float) + 32;
+    size_t smem = (size_t)rs_cta_floats(S) * sizeof(float);
     ps = s->profiling ? prof_slot(s, "k_pgs") : -1;
     if (ps >= 0) prof_mark(s, ps, true);
-    k_pgs<<<(N + 3) / 4, 32, smem, s->stream>>>(S, kp);
+    k_pgs<<<(N + RS_CTA_ENVS - 1) / RS_CTA_ENVS, 32, smem, s->stream>>>(S, kp);
     if (ps >= 0) prof_mark(s, ps, false);
     s->launches += 2;
   }
@@ -961,6 +961,17 @@ int ag_get_pgs_trips(AgSim* s, int32_t* trips, int32_t* stream_floats) {
   DevGuard guard__(s->device);
   if (trips && d2h(s, trips, s->S.pgs_trips, sizeof(int) * s->S.N)) return -1;
   if (stream_floats && d2h(s, stream_floats, s->S.rs_nfloats, sizeof(int) * s->S.N)) return -1;
+  return 0;
+}
+int ag_get_pgs_occupancy(AgSim* s, int32_t* ctas_per_sm, int32_t* smem_bytes) {
+  DevGuard guard__(s->device);
+  const size_t smem = (size_t)rs_cta_floats(s->S) * sizeof(float);
+  int ctas = 0;
+#ifndef AG_CPU_EMU
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas, k_pgs, 32, smem) != cudaSuccess) return fail("cudaOccupancyMaxActiveBlocksPerMultiprocessor(k_pgs) failed");
+#endif
+  if (ctas_per_sm) *ctas_per_sm = ctas;
+  if (smem_bytes) *smem_bytes = (int32_t)smem;
   return 0;
 }
 

@@ -181,6 +181,12 @@ class BatchSim:
         self._ck(self.lib.ag_get_pgs_trips(self.h, _p(t), _p(f)))
         return t, f
 
+    def pgs_occupancy(self):
+        """(PGS CTAs resident per SM, shared memory per PGS CTA in bytes)."""
+        c, b = C.c_int32(0), C.c_int32(0)
+        self._ck(self.lib.ag_get_pgs_occupancy(self.h, C.byref(c), C.byref(b)))
+        return c.value, b.value
+
     def profile_enable(self, on=True):
         self._ck(self.lib.ag_profile_enable(self.h, int(bool(on))))
 

@@ -380,6 +380,9 @@ int      ag_get_solver_stats(AgSim* sim, int32_t* contacts, int32_t* iters);
 /* SM cycles each env's lane spent inside the PGS kernel of the last substep (load-balance diagnostic) */
 int      ag_get_pgs_cycles(AgSim* sim, int32_t* cycles);           /* diagnostic: SM cycles each env spent in the last PGS launch */
 int      ag_get_pgs_trips(AgSim* sim, int32_t* trips, int32_t* stream_floats);  /* diagnostic: records its warp consumed / floats of its row stream */
+/* diagnostic: CTAs of the PGS kernel resident per SM (the runtime's occupancy calculator; 0 without a device) and its
+   shared memory per CTA in bytes */
+int      ag_get_pgs_occupancy(AgSim* sim, int32_t* ctas_per_sm, int32_t* smem_bytes);
 
 #ifdef __cplusplus
 }

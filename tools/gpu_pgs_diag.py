@@ -16,6 +16,7 @@ for i in range(steps):
     sim.feeding_step_host(acts[i])
 cyc = sim.pgs_cycles().astype(np.float64); cnt, it = sim.solver_stats(); trips, fl = sim.pgs_trips()
 q = [50, 90, 99, 99.9]
+print('k_pgs: %d CTAs per SM, %d B of shared memory per CTA' % sim.pgs_occupancy())
 print('cycles: mean %.0f p50 %.0f p90 %.0f p99 %.0f p99.9 %.0f max %.0f' % (cyc.mean(), *np.percentile(cyc, q), cyc.max()))
 print('trips : mean %.0f p50 %.0f p90 %.0f p99 %.0f p99.9 %.0f max %d' % (trips.mean(), *np.percentile(trips, q), trips.max()))
 print('stream bytes: mean %.0f p50 %.0f p99 %.0f max %d' % (4 * fl.mean(), *np.percentile(4 * fl, [50, 99]), 4 * fl.max()))
