@@ -92,6 +92,17 @@ class AgScratchParams(C.Structure):
                 ('c_v', C.c_float), ('c_f', C.c_float), ('c_hf', C.c_float), ('task_success_threshold', C.c_float)]
 
 
+AG_COOP_MAXJ, AG_COOP_MAXC = 48, 10
+
+
+class AgCoopParams(C.Structure):
+    _fields_ = [('task', C.c_int32), ('human_body_m', C.c_int32), ('human_body_f', C.c_int32), ('n_joints', C.c_int32),
+                ('joint_links_m', C.c_int32 * AG_COOP_MAXJ), ('joint_links_f', C.c_int32 * AG_COOP_MAXJ),
+                ('joint_lower', C.c_double * AG_COOP_MAXJ), ('joint_upper', C.c_double * AG_COOP_MAXJ),
+                ('n_ctrl', C.c_int32), ('ctrl', C.c_int32 * AG_COOP_MAXC), ('motor_gain', C.c_float), ('motor_force', C.c_float),
+                ('mlp_slots', C.c_int32 * 4), ('mlp_sign', C.c_float), ('mlp_sizes', C.c_int32 * 5), ('mlp_act', C.c_int32 * 4)]
+
+
 class AgCamera(C.Structure):
     _fields_ = [('eye', C.c_float * 3), ('target', C.c_float * 3), ('up', C.c_float * 3), ('fov_deg', C.c_float), ('aspect', C.c_float),
                 ('near_', C.c_float), ('far_', C.c_float), ('width', C.c_int32), ('height', C.c_int32), ('light_dir', C.c_float * 3),
@@ -239,6 +250,10 @@ def load_library(path=None):
     lib.ag_scratch_init.argtypes = [vp, C.POINTER(AgScratchParams), vp, vp, vp]
     lib.ag_scratch_step_dev.argtypes = [vp, vp, vp, vp, vp, vp]
     lib.ag_scratch_step_host.argtypes = [vp, vp, vp, vp, vp, vp]
+    lib.ag_coop_init.argtypes = [vp, C.POINTER(AgCoopParams), vp, vp]
+    lib.ag_coop_step_dev.argtypes = [vp, vp, vp, vp, vp, vp, vp]
+    lib.ag_coop_step_host.argtypes = [vp, vp, vp, vp, vp, vp, vp]
+    lib.ag_coop_classify.argtypes = [vp, ci, vp, vp]
     lib.ag_render.argtypes = [vp, C.POINTER(AgCamera), ci, vp, vp, vp]
     lib.ag_ik_solve.argtypes = [vp, ci, vp, ci, vp, vp, ci, ci, C.c_float, C.c_uint64, vp, vp, vp]
     lib.ag_state_size.restype = C.c_size_t
@@ -270,4 +285,5 @@ EXPORTED_SYMBOLS = [
     'ag_cloth_init', 'ag_cloth_set_state', 'ag_cloth_get_state', 'ag_cloth_set_anchor', 'ag_cloth_anchor_follow', 'ag_cloth_set_gravity',
     'ag_cloth_get_contacts', 'ag_cloth_device_state', 'ag_scratch_init', 'ag_scratch_step_dev', 'ag_scratch_step_host', 'ag_render', 'ag_set_body_gravity', 'ag_get_link_aabb', 'ag_dressing_init', 'ag_dressing_reset_episode', 'ag_dressing_set_tremor', 'ag_set_motor_force_scale', 'ag_dressing_step_dev', 'ag_dressing_step_host',
     'ag_overflow_count', 'ag_get_solver_stats', 'ag_get_pgs_cycles', 'ag_get_pgs_trips', 'ag_get_pgs_occupancy', 'ag_profile_enable', 'ag_profile_get',
+    'ag_coop_init', 'ag_coop_step_dev', 'ag_coop_step_host', 'ag_coop_classify',
 ]

@@ -144,11 +144,11 @@ AG_HDN inline void closest_body(int e, const SimDev& S, const KP& p) {
 }
 
 // ------------------------------------------------------------------ fused FeedingEnv
-// action -> PD targets.  p0 = action [N][7] (env-major), p1 = FeedDev*
+// action -> PD targets.  p0 = action [N][7 + i0] (env-major; the robot's 7 come first), p1 = FeedDev*
 AG_HDN inline void feeding_pre_body(int e, const SimDev& S, const KP& p) {
   const int N = S.N;
   const FeedDev& F = *(const FeedDev*)p.p1;
-  const float* act = (const float*)p.p0 + (size_t)e * 7;
+  const float* act = (const float*)p.p0 + (size_t)e * (7 + p.i0);
   F.iteration[e] += 1;
   for (int j = 0; j < 7; j++) {
     float raw = act[j];
@@ -205,7 +205,8 @@ AG_HD unsigned long long xorshift64s(unsigned long long& s) {
 }
 AG_HD float rng_uniform(unsigned long long& s) { return (float)(xorshift64s(s) >> 40) * (1.0f / 16777216.0f); }
 
-// obs / reward / done.  p0 = action, p1 = FeedDev*, p2 = obs [N][25], p3 = reward, p4 = done, p5 = info [N][4]
+// obs / reward / done.  p0 = action [N][7 + i0], p1 = FeedDev*, p2 = obs [N][25], p3 = reward, p4 = done, p5 = info [N][4].
+// The reward's action term is the norm of the whole raw action row (the person's i0 entries too, step_reference_api).
 AG_HDN inline void feeding_post_body(int e, const SimDev& S, const KP& p) {
   const int N = S.N;
   const FeedDev& F = *(const FeedDev*)p.p1;
@@ -297,6 +298,7 @@ AG_HDN inline void feeding_post_body(int e, const SimDev& S, const KP& p) {
   float pref = P.c_v * r_vel + P.c_f * r_nontarget + P.c_hf * r_high + P.c_fd * food_hit + P.c_fdv * (-vel_sum);
   float an = 0.f;
   for (int j = 0; j < 7; j++) { float a = F.action[(size_t)j * N + e]; an += a * a; }
+  for (int j = 0; j < p.i0; j++) { float a = ((const float*)p.p0)[(size_t)e * (7 + p.i0) + 7 + j]; an += a * a; }
   float reward = P.w_distance * (-norm(target - sp)) + P.w_action * (-sqrtf(an)) + P.w_food * food_reward + pref;
   ((float*)p.p3)[e] = reward;
   ((float*)p.p4)[e] = F.iteration[e] >= 200 ? 1.f : 0.f;

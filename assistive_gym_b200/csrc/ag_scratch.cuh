@@ -15,10 +15,11 @@ struct ScratchDev {
   float* action;                  // [7][N]
 };
 
+// p0 = action [N][7 + i0] (env-major; the robot's 7 come first), p1 = ScratchDev*
 AG_HDN inline void scratch_pre_body(int e, const SimDev& S, const KP& p) {
   const int N = S.N;
   const ScratchDev& D = *(const ScratchDev*)p.p1;
-  const float* act = (const float*)p.p0 + (size_t)e * 7;
+  const float* act = (const float*)p.p0 + (size_t)e * (7 + p.i0);
   D.iteration[e] += 1;
   for (int j = 0; j < 7; j++) {
     float raw = act[j];
@@ -36,7 +37,7 @@ AG_HDN inline void scratch_pre_body(int e, const SimDev& S, const KP& p) {
   }
 }
 
-// p0 = action, p1 = ScratchDev*, p2 = obs [N][30], p3 = reward, p4 = done, p5 = info [N][4] = total force on the person, task
+// p0 = action [N][7 + i0] (the reward's action term covers the whole raw row), p1 = ScratchDev*, p2 = obs [N][30], p3 = reward, p4 = done, p5 = info [N][4] = total force on the person, task
 // success, tool force at the target, scratches so far
 AG_HDN inline void scratch_post_body(int e, const SimDev& S, const KP& p) {
   const int N = S.N;
@@ -100,6 +101,7 @@ AG_HDN inline void scratch_post_body(int e, const SimDev& S, const KP& p) {
   float pref = P.c_v * (-norm(lin)) + P.c_f * (-(total_on_human - at_target)) + P.c_hf * (at_target < 10.f ? 0.f : -at_target);
   float an = 0.f;
   for (int j = 0; j < 7; j++) { float a = D.action[(size_t)j * N + e]; an += a * a; }
+  for (int j = 0; j < p.i0; j++) { float a = ((const float*)p.p0)[(size_t)e * (7 + p.i0) + 7 + j]; an += a * a; }
   ((float*)p.p3)[e] = P.w_distance * (-norm(target - tp)) + P.w_action * (-sqrtf(an)) + P.w_scratch * scratch + pref;
   ((float*)p.p4)[e] = D.iteration[e] >= 200 ? 1.f : 0.f;
   float* info = (float*)p.p5 + (size_t)e * 4;

@@ -18,6 +18,7 @@
 #include "ag_dressing.cuh"
 #include "ag_render.cuh"
 #include "ag_scratch.cuh"
+#include "ag_coop.cuh"
 
 #ifndef AG_CPU_EMU
 #include <cuda_runtime.h>
@@ -113,6 +114,49 @@ AG_KERNEL(k_scratch_post, scratch_post_body)
 AG_KERNEL(k_render, render_body)
 AG_KERNEL(k_cloth_snap, cloth_snap_body)
 AG_KERNEL(k_cloth_follow, cloth_follow_body)
+AG_KERNEL(k_coop_pre, coop_pre_body)
+AG_KERNEL(k_coop_obs, coop_obs_body)
+// k_coop_limits: one thread per env; the classifier's weights and a 2 x 64-float activation column per thread live in shared
+// memory (the weights only when the classifier is on).  k_coop_classify: the same classifier on a list of inputs.
+#define AG_COOP_T 64
+#ifndef AG_CPU_EMU
+__global__ void __launch_bounds__(AG_COOP_T) k_coop_limits(SimDev S, KP p) {
+  extern __shared__ __align__(16) float coop_smem[];
+  const CoopDev& C = *(const CoopDev*)p.p1;
+  if (C.mlp_on) {
+    for (int i = threadIdx.x; i < AG_MLP_FLOATS; i += blockDim.x) coop_smem[i] = C.mlp[i];
+    __syncthreads();
+  }
+  int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e < p.n) coop_limits_body(e, S, C, coop_smem, coop_smem + AG_MLP_FLOATS + threadIdx.x, blockDim.x);
+}
+__global__ void __launch_bounds__(AG_COOP_T) k_coop_classify(SimDev, KP p) {
+  extern __shared__ __align__(16) float coop_smem[];
+  const float* w = (const float*)p.p2;
+  for (int i = threadIdx.x; i < AG_MLP_FLOATS; i += blockDim.x) coop_smem[i] = w[i];
+  __syncthreads();
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < p.n) {
+    const float* xi = (const float*)p.p0 + (size_t)i * 4;
+    float x[4] = {xi[0], xi[1], xi[2], xi[3]};
+    ((float*)p.p3)[i] = coop_mlp(coop_smem, x, coop_smem + AG_MLP_FLOATS + threadIdx.x, blockDim.x);
+  }
+}
+#else
+static void k_coop_limits(SimDev S, KP p) {
+  const CoopDev& C = *(const CoopDev*)p.p1;
+  float h[2 * AG_MLP_H];
+  for (int e = 0; e < p.n; e++) coop_limits_body(e, S, C, C.mlp, h, 1);
+}
+static void k_coop_classify(SimDev, KP p) {
+  float h[2 * AG_MLP_H];
+  for (int i = 0; i < p.n; i++) {
+    const float* xi = (const float*)p.p0 + (size_t)i * 4;
+    float x[4] = {xi[0], xi[1], xi[2], xi[3]};
+    ((float*)p.p3)[i] = coop_mlp((const float*)p.p2, x, h, 1);
+  }
+}
+#endif
 
 // ------------------------------------------------------------------ host object
 struct AgSim {
@@ -142,9 +186,13 @@ struct AgSim {
   float *h_spin_in, *h_spin_out, *d_saction, *d_sobs, *d_sreward, *d_sdone, *d_sinfo;
   size_t render_pix; int render_n; int* d_render_ids; unsigned char* d_render_rgba; float* d_render_depth; void* d_render_dev;
   float *h_dpin_in, *h_dpin_out, *d_daction, *d_dobs, *d_dreward, *d_ddone, *d_dinfo;
+  // co-optimisation (the person's half; the robot's half is the feeding / scratch state above)
+  CoopDev CO; CoopDev* CO_dev; bool coop; int coop_width;
+  float *d_caction, *d_cobs_r, *d_cobs_h, *d_creward, *d_cdone, *d_cinfo;
+  float* coop_obs_h;                   // the human-obs buffer the captured coop step writes (not part of the graph key)
   // CUDA-graph replay of the fused env step (one graph per entry point, keyed by its device pointers)
   bool use_graph; int graph_failures;
-  struct StepGraph { void* exec; const void* key[5]; uint64_t launches; bool valid; } graphs[4];
+  struct StepGraph { void* exec; const void* key[5]; uint64_t launches; bool valid; } graphs[5];
   // profiling
   bool profiling;
   std::vector<std::string> knames;
@@ -299,7 +347,7 @@ AgSim* ag_create(const AgSceneDesc* d, const AgConfig* cfg, int n_envs, int devi
   AgSim* s = new AgSim();
   memset(&s->S, 0, sizeof(SimDev));
   memset(&s->F, 0, sizeof(FeedDev));
-  s->cfg = *cfg; s->device = device; s->launches = 0; s->feeding = false; s->bathing = false; s->cloth = false; s->cloth_sub = 0; s->C_dev = nullptr; s->dressing = false; s->DP_dev = nullptr; s->scratch = false; s->SD_dev = nullptr; s->graphs[3].valid = false; s->render_pix = 0; s->render_n = 0; s->d_render_ids = nullptr; s->d_render_rgba = nullptr; s->d_render_depth = nullptr; s->d_render_dev = nullptr; s->graphs[2].valid = false; s->use_graph = true; s->graph_failures = 0; s->graphs[0].valid = s->graphs[1].valid = false; s->B_dev = nullptr; s->stream = nullptr; s->F_dev = nullptr; s->profiling = false;
+  s->cfg = *cfg; s->device = device; s->launches = 0; s->feeding = false; s->bathing = false; s->cloth = false; s->cloth_sub = 0; s->C_dev = nullptr; s->dressing = false; s->DP_dev = nullptr; s->scratch = false; s->SD_dev = nullptr; s->graphs[3].valid = false; s->render_pix = 0; s->render_n = 0; s->d_render_ids = nullptr; s->d_render_rgba = nullptr; s->d_render_depth = nullptr; s->d_render_dev = nullptr; s->graphs[2].valid = false; s->use_graph = true; s->graph_failures = 0; s->graphs[0].valid = s->graphs[1].valid = false; s->graphs[4].valid = false; s->coop = false; s->CO_dev = nullptr; s->coop_obs_h = nullptr; s->B_dev = nullptr; s->stream = nullptr; s->F_dev = nullptr; s->profiling = false;
   s->d_stage = nullptr; s->stage_floats = 0;
 #ifndef AG_CPU_EMU
   { int ndev = 0; if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) { g_err = "no such CUDA device (is a CUDA device present? there is no CPU fallback)"; delete s; return nullptr; } }
@@ -547,7 +595,7 @@ void ag_destroy(AgSim* s) {
   if (s->bathing) { cudaFreeHost(s->h_bpin_in); cudaFreeHost(s->h_bpin_out); }
   if (s->dressing) { cudaFreeHost(s->h_dpin_in); cudaFreeHost(s->h_dpin_out); }
   if (s->scratch) { cudaFreeHost(s->h_spin_in); cudaFreeHost(s->h_spin_out); }
-  for (int g = 0; g < 4; g++) if (s->graphs[g].valid) cudaGraphExecDestroy((cudaGraphExec_t)s->graphs[g].exec);
+  for (int g = 0; g < 5; g++) if (s->graphs[g].valid) cudaGraphExecDestroy((cudaGraphExec_t)s->graphs[g].exec);
   if (s->stream) cudaStreamDestroy(s->stream);
 #else
   for (void* p : s->allocs) free(p);
@@ -725,7 +773,7 @@ int ag_set_motor_force_scale(AgSim* s, int n, const int32_t* links, const float*
     if (!s->S.motor_fscale) return fail("device allocation failed");
     std::vector<float> ones(cnt, 1.0f);
     if (h2d(s, s->S.motor_fscale, ones.data(), cnt * sizeof(float))) return -1;
-    for (int g = 0; g < 4; g++) drop_graph(s, g);        // captured kernels hold the SimDev of before (null pointer)
+    for (int g = 0; g < 5; g++) drop_graph(s, g);        // captured kernels hold the SimDev of before (null pointer)
   }
   return scatter_host(s, s->S.motor_fscale, 1, n, links, scale, nullptr);
 }
@@ -1008,8 +1056,9 @@ static int run_step(AgSim* s, int which, StepEnqueue enq, const float* action, f
   if (s->use_graph && !s->profiling) {
     // The graph is captured against the sim's OWN action buffer: a learner hands in a freshly allocated action tensor
     // every step, and a graph keyed on that address would be re-captured (~90 launches + instantiate) each time.
-    float* own = which == 0 ? s->d_action : (which == 1 ? s->d_baction : (which == 2 ? s->d_daction : s->d_saction));
-    if (action != own) { CK(cudaMemcpyAsync(own, action, sizeof(float) * 7 * s->S.N, cudaMemcpyDeviceToDevice, s->stream)); action = own; }
+    float* own = which == 0 ? s->d_action : (which == 1 ? s->d_baction : (which == 2 ? s->d_daction : (which == 3 ? s->d_saction : s->d_caction)));
+    const size_t width = which == 4 ? (size_t)s->coop_width : 7;
+    if (action != own) { CK(cudaMemcpyAsync(own, action, sizeof(float) * width * s->S.N, cudaMemcpyDeviceToDevice, s->stream)); action = own; }
     AgSim::StepGraph& G = s->graphs[which];
     const void* key[5] = {action, obs, reward, done, info};
     if (G.valid && memcmp(G.key, key, sizeof(key)) != 0) { cudaGraphExecDestroy((cudaGraphExec_t)G.exec); G.valid = false; }
@@ -1382,7 +1431,7 @@ int ag_scratch_init(AgSim* s, const AgScratchParams* p, const int32_t* gender_is
   for (int e = 0; e < N; e++) if (limb_link[e] < 0 || limb_link[e] >= s->nl) return fail("ag_scratch_init: bad limb link");
   ScratchDev& D = s->SD;
   D.P = *p;
-  drop_graph(s, 3);
+  drop_graph(s, 3); drop_graph(s, 4);
   if (!s->scratch) {
     D.male = dalloc<int>(s, N); D.iteration = dalloc<int>(s, N); D.task_success = dalloc<int>(s, N); D.limb_link = dalloc<int>(s, N);
     D.target_local = dalloc<float>(s, (size_t)3 * N); D.prev_contact = dalloc<float>(s, (size_t)3 * N); D.action = dalloc<float>(s, (size_t)7 * N);
@@ -1459,7 +1508,7 @@ int ag_feeding_init(AgSim* s, const AgFeedingParams* p, const int32_t* gender_is
   FeedDev& F = s->F;
   F.P = *p;
   if (p->n_foods > 16) return fail("too many foods");
-  drop_graph(s, 0);           // the captured step refers to the previous FeedDev
+  drop_graph(s, 0); drop_graph(s, 4);    // the captured steps refer to the previous FeedDev
   if (!s->feeding) {          // buffers are allocated once; a later init (episode reset) only refreshes their contents
     F.male = dalloc<int>(s, N); F.food_state = dalloc<int>(s, N); F.iteration = dalloc<int>(s, N); F.task_success = dalloc<int>(s, N);
     F.food_near = dalloc<int>(s, (size_t)N * 16);
@@ -1679,6 +1728,158 @@ int ag_bathing_step_host(AgSim* s, const float* action, float* obs, float* rewar
   memcpy(done, s->h_bpin_out + (size_t)N * 25, sizeof(float) * N);
   if (info) memcpy(info, s->h_bpin_out + (size_t)N * 26, sizeof(float) * N * 4);
   return 0;
+}
+
+// ------------------------------------------------------------------ fused co-optimisation path (ag_coop.cuh)
+static size_t coop_smem_bytes(bool mlp) { return mlp ? (size_t)(AG_MLP_FLOATS + 2 * AG_MLP_H * AG_COOP_T) * sizeof(float) : 0; }
+
+int ag_coop_init(AgSim* s, const AgCoopParams* p, const double* limit_scale, const float* mlp) {
+  DevGuard guard__(s->device);
+  const int N = s->S.N;
+  if (!p) return fail("ag_coop_init: bad arguments");
+  if (p->task == 0) {
+    if (!s->feeding) return fail("ag_coop_init: call ag_feeding_init first");
+    if (p->n_ctrl != 4) return fail("ag_coop_init: the feeding person has 4 controllable joints");
+  } else if (p->task == 1) {
+    if (!s->scratch) return fail("ag_coop_init: call ag_scratch_init first");
+    if (p->n_ctrl != 10) return fail("ag_coop_init: the scratch-itch person has 10 controllable joints");
+  } else return fail("ag_coop_init: task must be 0 (feeding) or 1 (scratch itch)");
+  if (p->human_body_m < 0 || p->human_body_m >= s->nb || p->human_body_f < 0 || p->human_body_f >= s->nb) return fail("ag_coop_init: bad body");
+  if (p->n_joints < 1 || p->n_joints > AG_COOP_MAXJ) return fail("ag_coop_init: 1..48 joints");
+  for (int j = 0; j < p->n_joints; j++) {
+    const int km = p->joint_links_m[j], kf = p->joint_links_f[j];
+    if (km < 0 || km >= s->nl || kf < 0 || kf >= s->nl || s->link_body[km] != p->human_body_m || s->link_body[kf] != p->human_body_f)
+      return fail("ag_coop_init: bad joint link");
+  }
+  for (int c = 0; c < p->n_ctrl; c++) if (p->ctrl[c] < 0 || p->ctrl[c] >= p->n_joints) return fail("ag_coop_init: bad controllable joint");
+  if (mlp) {
+    static const int sizes[5] = {4, AG_MLP_H, AG_MLP_H, AG_MLP_H, 1}, acts[4] = {1, 1, 1, 2};
+    for (int l = 0; l < 5; l++) if (p->mlp_sizes[l] != sizes[l]) return fail("ag_coop_init: the classifier must be 4-64-64-64-1");
+    for (int l = 0; l < 4; l++) if (p->mlp_act[l] != acts[l]) return fail("ag_coop_init: the classifier must be tanh, tanh, tanh, sigmoid");
+    for (int k = 0; k < 4; k++) if (p->mlp_slots[k] < 0 || p->mlp_slots[k] >= p->n_joints) return fail("ag_coop_init: bad classifier joint");
+    if (p->mlp_sign != 1.f && p->mlp_sign != -1.f) return fail("ag_coop_init: mlp_sign must be +1 or -1");
+  }
+  std::vector<double> sc(N, 1.0);
+  if (limit_scale) for (int e = 0; e < N; e++) {
+    if (!(limit_scale[e] > 0.0 && limit_scale[e] <= 1.0)) return fail("ag_coop_init: limit_scale must be in (0, 1]");
+    sc[e] = limit_scale[e];
+  }
+  drop_graph(s, 4);
+  CoopDev& C = s->CO;
+  if (!s->coop) {             // buffers are allocated once; a later init (episode reset) only refreshes their contents
+    C.limit_scale = dalloc<double>(s, N); C.prev_pose = dalloc<float>(s, (size_t)4 * N);
+    C.mlp = dalloc<float>(s, AG_MLP_FLOATS);
+    s->d_caction = dalloc<float>(s, (size_t)N * (7 + AG_COOP_MAXC));
+    s->d_cobs_r = dalloc<float>(s, (size_t)N * 30); s->d_cobs_h = dalloc<float>(s, (size_t)N * 34);
+    s->d_creward = dalloc<float>(s, N); s->d_cdone = dalloc<float>(s, N); s->d_cinfo = dalloc<float>(s, (size_t)N * 4);
+    s->CO_dev = dalloc<CoopDev>(s, 1);
+    if (!s->d_cinfo || !s->CO_dev) return fail("device allocation failed");
+#ifndef AG_CPU_EMU
+    CK(cudaFuncSetAttribute(k_coop_limits, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)coop_smem_bytes(true)));
+    CK(cudaFuncSetAttribute(k_coop_classify, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)coop_smem_bytes(true)));
+#endif
+  }
+  C.P = *p;
+  C.frame_skip = p->task == 0 ? s->F.P.frame_skip : s->SD.P.frame_skip;
+  C.male = p->task == 0 ? s->F.male : s->SD.male;
+  C.mlp_on = mlp != nullptr;
+  std::vector<float> none((size_t)4 * N, nanf(""));
+  if (h2d(s, C.limit_scale, sc.data(), sizeof(double) * N) || h2d(s, C.prev_pose, none.data(), sizeof(float) * 4 * N)) return -1;
+  if (mlp && h2d(s, (void*)C.mlp, mlp, sizeof(float) * AG_MLP_FLOATS)) return -1;
+  if (h2d(s, s->CO_dev, &C, sizeof(CoopDev))) return -1;
+  // take_step's control() re-issues the person's gains / forces every step; the first step would set these anyway
+  std::vector<int32_t> links; std::vector<float> kp, kd, mf;
+  for (int c = 0; c < p->n_ctrl; c++)
+    for (int g = 0; g < 2; g++) {
+      links.push_back(g ? p->joint_links_f[p->ctrl[c]] : p->joint_links_m[p->ctrl[c]]);
+      kp.push_back(p->motor_gain); kd.push_back(1.f); mf.push_back(p->motor_force);
+    }
+  if (ag_set_motor_host(s, (int)links.size(), links.data(), 1, nullptr, kp.data(), kd.data(), mf.data())) return -1;
+  s->coop_width = 7 + p->n_ctrl;
+  s->coop = true;
+  return 0;
+}
+static void coop_limits_launch(AgSim* s) {
+  KP p = kp0(); p.n = s->S.N; p.p1 = s->CO_dev;
+#ifndef AG_CPU_EMU
+  int ps = s->profiling ? prof_slot(s, "k_coop_limits") : -1;
+  if (ps >= 0) prof_mark(s, ps, true);
+  k_coop_limits<<<(p.n + AG_COOP_T - 1) / AG_COOP_T, AG_COOP_T, coop_smem_bytes(s->CO.mlp_on), s->stream>>>(s->S, p);
+  if (ps >= 0) prof_mark(s, ps, false);
+#else
+  k_coop_limits(s->S, p);
+#endif
+  s->launches++;
+}
+static int coop_step_enqueue(AgSim* s, const float* action_dev, float* obs, float* reward, float* done, float* info) {
+  const int N = s->S.N, k = s->CO.P.n_ctrl;
+  const bool feed = s->CO.P.task == 0;
+  void* task_dev = feed ? (void*)s->F_dev : (void*)s->SD_dev;
+  KP p = kp0(); p.p0 = action_dev; p.p1 = task_dev; p.i0 = k;
+  if (feed) LAUNCH(s, k_feed_pre, N, p); else LAUNCH(s, k_scratch_pre, N, p);
+  KP c = kp0(); c.p0 = action_dev; c.p1 = s->CO_dev;
+  LAUNCH(s, k_coop_pre, N, c);
+  const int sub = s->cfg.num_substeps > 0 ? s->cfg.num_substeps : 1;
+  for (int f = 0; f < s->CO.frame_skip; f++) {         // stepSimulation, then the person's limits (env.py:223-231)
+    for (int i = 0; i < sub; i++) substep(s);
+    coop_limits_launch(s);
+  }
+  KP z = kp0();
+  LAUNCH(s, k_fk, (size_t)s->S.nb * N, z);
+  KP q = kp0(); q.p0 = action_dev; q.p1 = task_dev; q.p2 = obs; q.p3 = reward; q.p4 = done; q.p5 = info; q.i0 = k;
+  if (feed) {
+    KP a = kp0(); a.p0 = s->S.movcol; a.i0 = s->S.nmovcol;
+    LAUNCH(s, k_aabb, (size_t)s->S.nmovcol * N, a);
+    KP l = kp0(); l.p0 = s->S.movlink; l.i0 = s->S.nmovlink;
+    LAUNCH(s, k_linkaabb, (size_t)s->S.nmovlink * N, l);
+    KP f = kp0(); f.p1 = s->F_dev;
+    LAUNCH(s, k_feed_food, (size_t)N * s->F.P.n_foods, f);
+    LAUNCH(s, k_feed_post, N, q);
+  } else {
+    LAUNCH(s, k_scratch_post, N, q);
+  }
+  KP o = kp0(); o.p1 = s->CO_dev; o.p2 = task_dev; o.p3 = s->coop_obs_h; o.p4 = info;
+  LAUNCH(s, k_coop_obs, N, o);
+  return 0;
+}
+int ag_coop_step_dev(AgSim* s, const float* action_dev, float* obs_robot_dev, float* obs_human_dev, float* reward_dev, float* done_dev, float* info_dev) {
+  DevGuard guard__(s->device);
+  if (!s->coop) return fail("ag_coop_init not called");
+  if (obs_human_dev != s->coop_obs_h) { drop_graph(s, 4); s->coop_obs_h = obs_human_dev; }
+  int rc = run_step(s, 4, coop_step_enqueue, action_dev, obs_robot_dev, reward_dev, done_dev, info_dev);
+#ifndef AG_CPU_EMU
+  CK(cudaGetLastError());
+#endif
+  return rc;
+}
+int ag_coop_step_host(AgSim* s, const float* action, float* obs_robot, float* obs_human, float* reward, float* done, float* info) {
+  DevGuard guard__(s->device);
+  if (!s->coop) return fail("ag_coop_init not called");
+  const int N = s->S.N;
+  const size_t ro = s->CO.P.task == 0 ? 25 : 30, ho = s->CO.P.task == 0 ? 23 : 34;
+  if (h2d(s, s->d_caction, action, sizeof(float) * N * s->coop_width)) return -1;
+  if (ag_coop_step_dev(s, s->d_caction, s->d_cobs_r, s->d_cobs_h, s->d_creward, s->d_cdone, s->d_cinfo)) return -1;
+  if (d2h(s, obs_robot, s->d_cobs_r, sizeof(float) * N * ro) || d2h(s, obs_human, s->d_cobs_h, sizeof(float) * N * ho) ||
+      d2h(s, reward, s->d_creward, sizeof(float) * N) || d2h(s, done, s->d_cdone, sizeof(float) * N)) return -1;
+  return info ? d2h(s, info, s->d_cinfo, sizeof(float) * N * 4) : 0;
+}
+int ag_coop_classify(AgSim* s, int n, const float* x, float* p) {
+  DevGuard guard__(s->device);
+  if (!s->coop || !s->CO.mlp_on) return fail("ag_coop_classify: ag_coop_init with a classifier first");
+  if (n < 0 || (n > 0 && (!x || !p))) return fail("ag_coop_classify: bad arguments");
+  if (n == 0) return 0;
+  float* st = stage(s, (size_t)n * 5);
+  if (!st) return fail("staging alloc failed");
+  if (h2d(s, st, x, sizeof(float) * 4 * n)) return -1;
+  KP k = kp0(); k.n = n; k.p0 = st; k.p2 = (void*)s->CO.mlp; k.p3 = st + (size_t)4 * n;
+#ifndef AG_CPU_EMU
+  k_coop_classify<<<(n + AG_COOP_T - 1) / AG_COOP_T, AG_COOP_T, coop_smem_bytes(true), s->stream>>>(s->S, k);
+  CK(cudaGetLastError());
+#else
+  k_coop_classify(s->S, k);
+#endif
+  s->launches++;
+  return d2h(s, p, st + (size_t)4 * n, sizeof(float) * n);
 }
 
 }  // extern "C"

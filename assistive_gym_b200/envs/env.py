@@ -208,6 +208,25 @@ class AssistiveEnv(gym.Env):
     def update_targets(self):
         pass
 
+    def _coop_step_fused(self, action):
+        """The co-optimisation step (dict action in, dict observations / rewards / dones / infos out, as `step` returns them with a
+        controllable person) on the fused device path: robot and person act, the person's limits and the realistic-arm-limit
+        classifier run on the device after every substep (ag_coop_step_host).  Armed by `reset` (`start_coop`)."""
+        if not (self.human is not None and self.human.controllable):
+            raise RuntimeError('step_fused is the co-optimisation step: this env has no controllable person')
+        n = self.n_envs
+        a = np.concatenate([np.asarray(action['robot'], dtype=np.float32).reshape(n, -1), np.asarray(action['human'], dtype=np.float32).reshape(n, -1)], axis=1)
+        obs_r, obs_h, rew, done, info = self.id.coop_step_host(a)
+        self.iteration += 1
+        self.total_force_on_human = info[:, 0].astype(np.float64)
+        sq = (lambda v: v[0] if n == 1 else v)
+        obs = {'robot': sq(obs_r.astype(np.float64)), 'human': sq(obs_h.astype(np.float64))}
+        reward, done = sq(rew.astype(np.float64)), sq(done > 0.5)
+        inf = {'total_force_on_human': self.total_force_on_human, 'task_success': info[:, 1].astype(int),
+               'action_robot_len': self.action_robot_len, 'action_human_len': self.action_human_len, 'obs_robot_len': self.obs_robot_len, 'obs_human_len': self.obs_human_len}
+        d = bool(np.all(done)) if n > 1 else bool(done)
+        return obs, {'robot': reward, 'human': reward}, {'robot': done, 'human': done, '__all__': d}, {'robot': inf, 'human': inf}
+
     # ---- env.py:237-274
     def human_preferences(self, end_effector_velocity=0, total_force_on_human=0, tool_force_at_target=0, food_hit_human_reward=0,
                           food_mouth_velocities=(), dressing_forces=((),), arm_manipulation_tool_forces_on_human=(0, 0),

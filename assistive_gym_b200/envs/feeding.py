@@ -1,7 +1,8 @@
 """`FeedingEnv` (reference envs/feeding.py) on the batched backend.
 
 `step` runs the fused kernels (`ag_feeding_step_host`): action -> PD targets -> 5 substeps -> obs /
-reward / done.  `step_reference_api` performs the same step the way the reference does it —
+reward / done.  With a controllable person (FeedingJacoHuman-v1) `step` goes through the per-call path and `step_fused` through
+the fused co-optimisation kernels (`ag_coop_step_host`).  `step_reference_api` performs the same step the way the reference does it —
 `take_step` + `_get_obs` + `get_food_rewards` + `human_preferences` through the per-call `Agent`
 API — and exists so that tests can show the two paths agree."""
 import numpy as np
@@ -84,6 +85,8 @@ class FeedingEnv(AssistiveEnv):
             self._feeding_ready = True
         else:
             fb.start_fused(self.id, s, seed=self._seed)
+        if coop:
+            fb.start_coop(self.id, s)
         self.foods = np.ones((self.n_envs, 8), dtype=bool)
         self.foods_active = np.ones((self.n_envs, 8), dtype=bool)
         self.task_success = np.zeros(self.n_envs, dtype=int)
@@ -112,6 +115,11 @@ class FeedingEnv(AssistiveEnv):
         if self.n_envs == 1:
             return obs[0], float(rew[0]), bool(done[0] > 0.5), infos[0]
         return obs, rew, done > 0.5, infos
+
+    def step_fused(self, action):
+        """`step` of the co-optimisation env (FeedingJacoHuman-v1) on the fused, graph-replayed device path: takes and returns
+        exactly what `step` does.  `step` itself stays on the per-call path."""
+        return self._coop_step_fused(action)
 
     # ------------------------------------------------------------------ the same step through the reference-shaped API
     def _head_pose(self):

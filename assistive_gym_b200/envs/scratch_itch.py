@@ -2,7 +2,8 @@
 (`ag_scratch_step_host`); `_get_obs` (used by `reset`) reads the same quantities through the per-call Agent API.
 With a controllable person (co-optimisation, `ScratchItchJacoHuman-v1`) `step` takes {'robot': a7, 'human': a10} and goes through
 the per-call path (`step_reference_api`): `take_step` drives the person's right arm too and keeps it inside the realistic joint
-limits (the MLP classifier of human.py:134-152) after every substep."""
+limits (the MLP classifier of human.py:134-152) after every substep.  `step_fused` runs the same co-optimisation step on the
+device (`ag_coop_step_host`)."""
 import numpy as np
 
 from .. import capi
@@ -38,10 +39,16 @@ class ScratchItchEnv(AssistiveEnv):
             return obs[0], float(rew[0]), bool(done[0] > 0.5), {k_: (v[0] if isinstance(v, np.ndarray) else v) for k_, v in out.items()}
         return obs, rew, done > 0.5, out
 
+    def step_fused(self, action):
+        """`step` of the co-optimisation env (ScratchItchJacoHuman-v1) on the fused, graph-replayed device path: takes and returns
+        exactly what `step` does.  `step` itself stays on the per-call path."""
+        return self._coop_step_fused(action)
+
     def update_targets(self):                                              # scratch_itch.py:149-153
-        ls = self.id.get_link_states(list(self._limb_links))
+        links, col = np.unique(self._limb_links, return_inverse=True)       # a handful of distinct links, whatever the batch size
+        ls = self.id.get_link_states(list(links))
         idx = np.arange(self.n_envs)
-        self.target_pos = ls['pos'][idx, idx].astype(np.float64) + q_rot(ls['quat'][idx, idx].astype(np.float64), self._target_local)
+        self.target_pos = ls['pos'][idx, col].astype(np.float64) + q_rot(ls['quat'][idx, col].astype(np.float64), self._target_local)
 
     def _get_obs(self, agent=None):                                        # scratch_itch.py:60-91
         self.update_targets()
@@ -149,6 +156,8 @@ class ScratchItchEnv(AssistiveEnv):
             self.id.forward_kinematics()
         self._limb_links, self._target_local = sb.limb_links(s), s['target_local']
         sb.start_fused(self.id, s)
+        if self.human.controllable:
+            sb.start_coop(self.id, s)
         self.task_success = np.zeros(self.n_envs, dtype=int)
         obs = self._get_obs()
         if isinstance(obs, dict):

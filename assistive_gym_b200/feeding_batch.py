@@ -32,6 +32,47 @@ HEAD_JOINTS = (21, 22, 23)
 HEAD_LINK = 23
 TREMOR_JOINTS = (20, 21, 22, 23)      # human.head_joints = the controllable joints of FeedingEnv (feeding_envs.py)
 IMPAIRMENTS = ('none', 'limits', 'weakness', 'tremor')
+MLP_ACT = {'tanh': 1, 'sigmoid': 2}
+
+
+def coop_params(scene, humans, task, ctrl, motor_gain, motor_force=1.0):
+    """AgCoopParams of a controllable person: every joint's global link per gender, its template limits as the per-call Agent
+    sees them (agent.py update_joint_limits: an unlimited joint is +-1e10), and the controllable joints (indices into that list)."""
+    P = capi.AgCoopParams()
+    P.task, P.human_body_m, P.human_body_f = task, humans['male'], humans['female']
+    nj = int(scene['body_nlinks'][humans['male']]) - 1
+    P.n_joints = nj
+    for g, hb in humans.items():
+        l0 = int(scene['body_link0'][hb])
+        links = P.joint_links_m if g == 'male' else P.joint_links_f
+        for j in range(nj):
+            links[j] = l0 + 1 + j
+    l0 = int(scene['body_link0'][humans['male']])
+    for j in range(nj):
+        lo, hi = float(scene['link_lower'][l0 + 1 + j]), float(scene['link_upper'][l0 + 1 + j])
+        if lo == 0 and hi == -1:
+            lo, hi = -1e10, 1e10
+        P.joint_lower[j], P.joint_upper[j] = lo, hi
+    P.n_ctrl = len(ctrl)
+    for c, j in enumerate(ctrl):
+        P.ctrl[c] = j
+    P.motor_gain, P.motor_force = motor_gain, motor_force
+    return P
+
+
+def pack_mlp(P, model, slots, sign):
+    """Arm the classifier in `P` and return limits_model.ArmLimitsModel's weights packed in the order of agphys.h."""
+    for k, j in enumerate(slots):
+        P.mlp_slots[k] = j
+    P.mlp_sign = sign
+    sizes = [model.layers[0][0].shape[0]] + [W.shape[1] for W, _, _ in model.layers]
+    if len(sizes) != 5:
+        raise ValueError('the joint-limit classifier must have 4 layers, not %d' % (len(sizes) - 1))
+    for k, n in enumerate(sizes):
+        P.mlp_sizes[k] = n
+    for k, (_, _, act) in enumerate(model.layers):
+        P.mlp_act[k] = MLP_ACT.get(act, 0)
+    return np.concatenate([np.concatenate([W.ravel(), b.ravel()]) for W, b, _ in model.layers]).astype(np.float32)
 
 
 class FeedingBatch:
@@ -119,6 +160,12 @@ class FeedingBatch:
         if imp is not None and np.any(imp == 3):
             rest = self.tremor_rest_of(s)
             sim.feeding_set_tremor((imp == 3).astype(np.int32), rest, s['tremors'])
+
+    def start_coop(self, sim, sample=None):
+        """Arm the person's half of the fused co-optimisation step (FeedingJacoHuman-v1); call after `start_fused`.  The head
+        joints are driven with the gains take_step re-issues every step (feeding.py:122: 0.025, human.py force 1.0); the
+        feeding person's limits are not scaled."""
+        sim.coop_init(coop_params(self.scene, self.humans, 0, TREMOR_JOINTS, 0.025))
 
     def tremor_rest_of(self, s):
         """target_joint_angles of the head joints (human.py:122): neck 0, head x/y/z the sampled pose, limit-clipped."""

@@ -10,6 +10,7 @@ import numpy as np
 
 from . import capi
 from .feeding_batch import JACO as FEED_JACO
+from .feeding_batch import coop_params, pack_mlp
 from .human_model import create_human
 from .kinematics import BodyKinematics, q_from_rpy, q_mul, q_rot
 from .scene import SceneBuilder, quat_from_rpy
@@ -18,6 +19,7 @@ MOTOR_POSITION = 1
 JACO = dict(FEED_JACO, gripper_pos=1.0, tool_pos_offset=[0, 0, 0.02], tool_orient_offset=[0, -np.pi / 2.0, 0], ee_orient_rpy=[0, np.pi / 2.0, 0])   # jaco.py:19-42
 RIGHT_ARM_JOINTS = list(range(0, 10))                    # human.right_arm_joints (scratch_itch_envs.py:15)
 R_SHOULDER, R_ELBOW, R_WRIST = 5, 7, 9
+R_ARM_LIMIT_JOINTS = [3, 4, 5, 6]                        # shoulder x, y, z and elbow: the classifier's inputs (human.py:137-140)
 HUMAN_PRESET = {3: 30, 6: -90, 16: -90, 28: -90, 31: 80, 35: -90, 38: 80}      # degrees, scratch_itch.py:104
 LIMBS = {'male': ((R_SHOULDER, 0.279, 0.043), (R_ELBOW, 0.257, 0.033)), 'female': ((R_SHOULDER, 0.264, 0.0355), (R_ELBOW, 0.234, 0.027))}   # scratch_itch.py:136-139
 
@@ -176,3 +178,14 @@ class ScratchItchBatch:
     def start_fused(self, sim, sample=None):
         s = sample or self.last_sample
         sim.scratch_init(self.scratch_params(), s['male'], self.limb_links(s), s['target_local'])
+
+    def start_coop(self, sim, sample=None):
+        """Arm the person's half of the fused co-optimisation step (ScratchItchJacoHuman-v1); call after `start_fused`.  The arm
+        is driven with Human.motor_gains / motor_forces (0.05, 1.0), which take_step re-issues every step in place of the reset's
+        0.01; the `weakness` force scale set by `reset` stays.  Limits are scaled by the sample's `limit_scale`; the right arm is
+        kept inside the realistic joint limits by the classifier of limits_model."""
+        from .limits_model import load_model
+        s = sample or self.last_sample
+        P = coop_params(self.scene, self.humans, 1, RIGHT_ARM_JOINTS, 0.05)
+        w = pack_mlp(P, load_model(), R_ARM_LIMIT_JOINTS, -1.0)
+        sim.coop_init(P, limit_scale=s.get('limit_scale'), mlp=w)

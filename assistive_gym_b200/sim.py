@@ -304,6 +304,36 @@ class BatchSim:
     def scratch_step_dev(self, action_ptr, obs_ptr, reward_ptr, done_ptr, info_ptr):
         self._ck(self.lib.ag_scratch_step_dev(self.h, action_ptr, obs_ptr, reward_ptr, done_ptr, info_ptr))
 
+    # ---- fused co-optimisation path (the person's half; call after feeding_init / scratch_init)
+    def coop_init(self, params, limit_scale=None, mlp=None):
+        """limit_scale [n] or None; mlp: the packed classifier weights (fp32, agphys.h order) or None"""
+        self._coop_params = params
+        self._coop_dims = (25, 23) if params.task == 0 else (30, 34)
+        ls = None if limit_scale is None else np.ascontiguousarray(np.broadcast_to(np.asarray(limit_scale, dtype=np.float64), (self.n,)))
+        w = None if mlp is None else np.ascontiguousarray(mlp, dtype=np.float32)
+        self._ck(self.lib.ag_coop_init(self.h, C.byref(params), _p(ls), _p(w)))
+
+    def coop_step_host(self, action):
+        """action [n, 7 + n_ctrl] (robot, then person) -> obs_robot, obs_human, reward, done, info [n, 4]"""
+        a = _f32(action, (self.n, 7 + int(self._coop_params.n_ctrl)))
+        ro, ho = self._coop_dims
+        obs_r, obs_h = np.empty((self.n, ro), dtype=np.float32), np.empty((self.n, ho), dtype=np.float32)
+        rew, done = np.empty(self.n, dtype=np.float32), np.empty(self.n, dtype=np.float32)
+        info = np.empty((self.n, 4), dtype=np.float32)
+        self._ck(self.lib.ag_coop_step_host(self.h, _p(a), _p(obs_r), _p(obs_h), _p(rew), _p(done), _p(info)))
+        return obs_r, obs_h, rew, done, info
+
+    def coop_step_dev(self, action_ptr, obs_robot_ptr, obs_human_ptr, reward_ptr, done_ptr, info_ptr):
+        self._ck(self.lib.ag_coop_step_dev(self.h, C.c_void_p(action_ptr), C.c_void_p(obs_robot_ptr), C.c_void_p(obs_human_ptr),
+                                           C.c_void_p(reward_ptr), C.c_void_p(done_ptr), C.c_void_p(info_ptr)))
+
+    def coop_classify(self, x):
+        """the device joint-limit classifier on x [m, 4] -> p [m]"""
+        x = _f32(x)
+        p = np.empty(len(x), dtype=np.float32)
+        self._ck(self.lib.ag_coop_classify(self.h, len(x), _p(x), _p(p)))
+        return p
+
     # ---- camera images (ag_render)
     def render(self, eye, target, fov=60.0, width=480, height=270, env_ids=(0,), up=(0, 0, 1), near=0.01, far=100.0,
                light_dir=(0, -3, 1), ambient=0.8, diffuse=0.3):

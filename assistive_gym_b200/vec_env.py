@@ -6,7 +6,11 @@ The reference trains one `gym.Env` per RLlib worker process (`learn.py:26,61-69`
 written into pre-allocated device tensors on the simulation's own stream, and nothing crosses PCIe.  Episodes of
 all envs have the same length (200 steps, feeding.py:37), so the batch resets together; `auto_reset` does it inside
 `step` the way vector-env wrappers do (the terminal observation is kept in `info['terminal_observation']`).
-With numpy inputs the host-buffer entry points are used instead (pinned staging inside the C ABI)."""
+With numpy inputs the host-buffer entry points are used instead (pinned staging inside the C ABI).
+
+The co-optimisation ids (FeedingJacoHuman-v1, ScratchItchJacoHuman-v1) run `ag_coop_step_dev`: actions are
+{'robot': [N, 7], 'human': [N, k]}, observations {'robot': [N, 25 | 30], 'human': [N, 23 | 34]}, and rewards, dones and infos
+come in the dict shape of the env's `step` (dones with '__all__')."""
 import numpy as np
 
 
@@ -30,13 +34,14 @@ class AssistiveVecEnv:
         self.task = self.env.task
         self.observation_space, self.action_space = self.env.observation_space, self.env.action_space
         self.obs_dim, self.act_dim = self.observation_space.shape[0], self.action_space.shape[0]
+        self.coop = self.task in ('feeding', 'scratch_itch') and bool(self.env.human.controllable)
         self._step_dev = None
         self._buf = None
 
     # ------------------------------------------------------------------ gym-style API
     def _reset_standby(self):
         try:
-            self._bg_obs = np.atleast_2d(self._standby.reset())
+            self._bg_obs = self._batch_obs(self._standby.reset())
         except Exception as ex:          # surfaced by the next reset()
             self._bg_err = ex
 
@@ -55,21 +60,32 @@ class AssistiveVecEnv:
             obs = self._bg_obs
             self._buf = None                                            # device tensors are bound to a sim's stream
         else:
-            obs = np.atleast_2d(self.env.reset())
+            obs = self._batch_obs(self.env.reset())
         if self._standby is not None:
             self._start_standby()
         sim = self.env.id
+        self._t = 0
+        if self.coop:
+            self._step_dev, self._step_host = sim.coop_step_dev, sim.coop_step_host
+            return obs
         self._step_dev = {'feeding': sim.feeding_step_dev, 'bed_bathing': sim.bathing_step_dev, 'dressing': sim.dressing_step_dev, 'scratch_itch': sim.scratch_step_dev}[self.task]
         self._step_host = {'feeding': sim.feeding_step_host, 'bed_bathing': sim.bathing_step_host, 'dressing': sim.dressing_step_host, 'scratch_itch': sim.scratch_step_host}[self.task]
-        self._t = 0
         return obs
+
+    def _batch_obs(self, obs):
+        if isinstance(obs, dict):
+            return {k: np.atleast_2d(v) for k, v in obs.items()}
+        return np.atleast_2d(obs)
 
     def _tensors(self, like):
         import torch
         if self._buf is None or self._buf[0].device != like.device:
             n = self.n_envs
             mk = lambda *shape: torch.zeros(shape, device=like.device, dtype=torch.float32)
-            self._buf = (mk(n, self.obs_dim), mk(n), mk(n), mk(n, 4))
+            if self.coop:
+                self._buf = (mk(n, self.env.obs_robot_len), mk(n, self.env.obs_human_len), mk(n), mk(n), mk(n, 4))
+            else:
+                self._buf = (mk(n, self.obs_dim), mk(n), mk(n), mk(n, 4))
             self._stream = torch.cuda.ExternalStream(self.env.id.stream_ptr(), device=like.device)
         return self._buf
 
@@ -77,6 +93,8 @@ class AssistiveVecEnv:
         """actions: torch CUDA tensor [n_envs, act_dim] (float32, contiguous) -> device tensors, or numpy -> numpy."""
         if self._step_dev is None:
             raise RuntimeError('call reset() first')
+        if self.coop:
+            return self._step_coop(actions)
         is_torch = hasattr(actions, 'data_ptr')
         if is_torch:
             import torch
@@ -101,6 +119,37 @@ class AssistiveVecEnv:
                 new_obs = torch.as_tensor(new_obs, device=out[0].device, dtype=torch.float32)
             out = (new_obs, out[1], out[2], dict(out[3], terminal_observation=term))
         return out
+
+    def _step_coop(self, actions):
+        """actions {'robot': [n, 7], 'human': [n, k]}: torch CUDA tensors -> device tensors, or numpy -> numpy"""
+        is_torch = hasattr(actions['robot'], 'data_ptr')
+        if is_torch:
+            import torch
+            a = torch.cat([actions['robot'].to(dtype=torch.float32), actions['human'].to(dtype=torch.float32)], dim=1).contiguous()
+            obs_r, obs_h, rew, done, info = self._tensors(a)
+            self._stream.wait_stream(torch.cuda.current_stream(a.device))
+            self._step_dev(a.data_ptr(), obs_r.data_ptr(), obs_h.data_ptr(), rew.data_ptr(), done.data_ptr(), info.data_ptr())
+            torch.cuda.current_stream(a.device).wait_stream(self._stream)
+        else:
+            a = np.concatenate([np.asarray(actions['robot'], dtype=np.float32).reshape(self.n_envs, -1),
+                                np.asarray(actions['human'], dtype=np.float32).reshape(self.n_envs, -1)], axis=1)
+            obs_r, obs_h, rew, done, info = self._step_host(a)
+        self._t += 1
+        self.env.iteration = self._t
+        d = done > 0.5
+        inf = {'total_force_on_human': info[:, 0], 'task_success': info[:, 1]}
+        obs = {'robot': obs_r, 'human': obs_h}
+        dones = {'robot': d, 'human': d, '__all__': self._t >= 200}       # every env's episode ends at step 200 (feeding.py:37)
+        infos = {'robot': inf, 'human': dict(inf)}
+        if self.auto_reset and self._t >= 200:
+            term = {k: (v.clone() if is_torch else v.copy()) for k, v in obs.items()}
+            new_obs = self.reset()
+            if is_torch:
+                import torch
+                new_obs = {k: torch.as_tensor(v, device=obs_r.device, dtype=torch.float32) for k, v in new_obs.items()}
+            obs = new_obs
+            infos = {k: dict(v, terminal_observation=term[k]) for k, v in infos.items()}
+        return obs, {'robot': rew, 'human': rew}, dones, infos
 
     def close(self):
         if self._bg is not None:
