@@ -15,9 +15,17 @@ Differences forced by lock-step batching or by what the backend does not simulat
     first draw whose start pose is reachable and collision-free is kept; the JLWKI manipulability ranking over
     50 draws (robot.py:150-186) is not restated (reset-time code, SURVEY.md §8(f)1);
   * the 91 / 129 target marker bodies (bed_bathing.py:187-188) are not instantiated: targets are points.
+
+With `controllable_person=True` (BedBathingSawyerHuman-v1) the person's right arm is a second agent: its ten joints keep their
+mass (`setup_joints(use_static_joints=True, reactive_force=None)` with a controllable person, human.py:104-127), the active
+gender is simulated instead of frozen, and the impairment is drawn with 'no_tremor' (as FeedingJacoHuman-v1 does, feeding.py:59).
+`tremor` is not built for a controllable person: the co-optimisation kernels keep no per-env rest angles.  `weakness` is drawn but
+does not act: the task sets no reactive force, and take_step's control() drives the arm with motor_forces 1.0.  The wiping targets
+then follow the arm (update_targets, bed_bathing.py:190-203), from their link frames (`target_frames`).
 """
 import numpy as np
 
+from .feeding_batch import coop_params, pack_mlp
 from .human_model import create_human
 from .kinematics import BodyKinematics, ik_dls, q_from_rpy, q_mul, q_rot
 from .toc import position_robot_toc
@@ -32,6 +40,8 @@ J_RIGHT_SHOULDER_X = 3
 # (upperarm length, radius, forearm length, radius), bed_bathing.py:176-181
 ARM_DIMS = {'male': (0.279, 0.043, 0.257, 0.033), 'female': (0.264, 0.0355, 0.234, 0.027)}
 WIPER_CLOTH_LINK = 1                             # `if linkA in [1]`, bed_bathing.py:49
+RIGHT_ARM_JOINTS = list(range(0, 10))            # human.right_arm_joints (bed_bathing_envs.py)
+R_ARM_LIMIT_JOINTS = [3, 4, 5, 6]                # shoulder x, y, z and elbow: the classifier's inputs (human.py:137-140)
 
 
 def orthogonal_vector(v):
@@ -62,7 +72,8 @@ def capsule_points(p1, p2, radius, distance_between_points=0.05):
 
 
 class BedBathingBatch:
-    def __init__(self):
+    def __init__(self, controllable_person=False):
+        self.controllable_person = bool(controllable_person)
         b = SceneBuilder()
         self.builder = b
         b.set_gravity([0, 0, -9.81])
@@ -73,7 +84,8 @@ class BedBathingBatch:
         for gender in ('male', 'female'):
             hb, info = create_human(b, gender=gender, static=True)
             for j in range(b.num_joints(hb)):                                    # "static joints" after the settle (bed_bathing.py:133-136)
-                b.change_dynamics(hb, j, mass=0)
+                if not (self.controllable_person and j in RIGHT_ARM_JOINTS):  # a controllable arm keeps its mass (human.py:108-112)
+                    b.change_dynamics(hb, j, mass=0)
             b.set_gravity([0, 0, -1], body=hb)
             self.humans[gender] = hb
         self.robot = b.load_urdf('sawyer', base_pos=[-1, -1, 0.975], fixed_base=True, self_collision=True)
@@ -109,6 +121,7 @@ class BedBathingBatch:
         for g, (ul, ur, fl, fr) in ARM_DIMS.items():
             self.targets_local[g] = (capsule_points([0, 0, 0], [0, 0, -ul], ur, 0.03), capsule_points([0, 0, 0], [0, 0, -fl], fr, 0.03))
         self.max_targets = max(len(u) + len(f) for u, f in self.targets_local.values())
+        self.human_arm_links = {g: [self.gl(hb, j) for j in RIGHT_ARM_JOINTS] for g, hb in self.humans.items()}
 
     # ------------------------------------------------------------------ params for the fused kernels
     def bathing_params(self):
@@ -142,15 +155,34 @@ class BedBathingBatch:
         sim.bathing_init(self.bathing_params(), s['male'], tw, valid)
         return tw, valid
 
+    def start_coop(self, sim, sample=None):
+        """Arm the person's half of the fused co-optimisation step (BedBathingSawyerHuman-v1); call after `start_fused`.  The
+        targets follow the arm from their link frames; the arm is driven with Human.motor_gains / motor_forces (0.05, 1.0), the
+        gains take_step's control() issues every step; limits are scaled by the sample's `limit_scale`; the classifier of
+        limits_model keeps the right arm inside the realistic joint limits."""
+        from .limits_model import load_model
+        s = sample or self.last_sample
+        link, local = self.target_frames(s)
+        sim.bathing_set_target_frames(link, local)
+        P = coop_params(self.scene, self.humans, 2, RIGHT_ARM_JOINTS, 0.05)
+        w = pack_mlp(P, load_model(), R_ARM_LIMIT_JOINTS, -1.0)
+        sim.coop_init(P, limit_scale=s.get('limit_scale'), mlp=w)
+
     # ------------------------------------------------------------------ batched reset
     def sample(self, n, rng):
         nj = 41
-        return dict(
+        s = dict(
             plane_friction=rng.uniform(0.025, 0.5, size=n),                       # env.py:120
             male=rng.integers(0, 2, size=n).astype(np.int32),
             joint_noise=rng.uniform(-0.1, 0.1, size=(n, nj)),                     # bed_bathing.py:126-127
             ee_offset=rng.uniform(-0.05, 0.05, size=(n, 3)),                      # bed_bathing.py:145
         )
+        if self.controllable_person:         # drawn after every other field, so that the static person's draws stay as they are
+            imp = rng.integers(0, 3, size=n)                                      # none / limits / weakness ('no_tremor', human.py:82-83)
+            s['impairment'] = imp.astype(np.int32)
+            s['limit_scale'] = np.where(imp == 1, rng.uniform(0.5, 1.0, size=n), 1.0)      # human.py:85
+            s['strength'] = np.where(imp == 2, rng.uniform(0.25, 1.0, size=n), 1.0)        # human.py:86 (drawn, no effect here)
+        return s
 
     def human_pose(self, s):
         """Joint angles of the lying person: right shoulder x 30 deg (bed_bathing.py:119), noise on every motor joint,
@@ -226,7 +258,8 @@ class BedBathingBatch:
             links, q = poses[g]
             sim.set_joint_state(links, q=q, qd=np.zeros_like(q))
             sim.set_base_pose(hb, hpos, np.tile(lie, (n, 1)))
-            sim.set_body_active(hb, np.where(male if g == 'male' else ~male, 2, 0).astype(np.int32))
+            # frozen (2), or simulated (1) when the person is controllable; no motors on the arm at reset (reactive_force=None)
+            sim.set_body_active(hb, np.where(male if g == 'male' else ~male, 1 if self.controllable_person else 2, 0).astype(np.int32))
         sim.forward_kinematics()
         drop = np.zeros(n)
         for g, hb in self.humans.items():
@@ -370,6 +403,21 @@ class BedBathingBatch:
             out[on, :w.shape[1]] = w[on]
             valid[on, :w.shape[1]] = True
         return out, valid
+
+    def target_frames(self, s):
+        """Per env the global link each target rides on (upper arm R_SHOULDER, forearm R_ELBOW; -1 for padding) [n, T] and the
+        target in that link's frame [n, T, 3], in the order of `targets_world`."""
+        male = np.asarray(s['male']).astype(bool)
+        n = len(male)
+        link = np.full((n, self.max_targets), -1, dtype=np.int32)
+        local = np.zeros((n, self.max_targets, 3))
+        for g, hb in self.humans.items():
+            on = male if g == 'male' else ~male
+            tu, tf = self.targets_local[g]
+            nu, nt = len(tu), len(tu) + len(tf)
+            link[on, :nu], link[on, nu:nt] = self.gl(hb, R_SHOULDER), self.gl(hb, R_ELBOW)
+            local[on, :nt] = np.concatenate([tu, tf], axis=0)
+        return link, local
 
     def total_force(self, sim, targets_pos_world, targets_alive, max_tool_contacts=32):
         """`BedBathingEnv.get_total_force` (bed_bathing.py:41-78) on any sim with the BatchSim getter surface: robot and

@@ -234,6 +234,7 @@ def load_library(path=None):
     lib.ag_bathing_init.argtypes = [vp, C.POINTER(AgBathingParams), vp, vp, vp]
     lib.ag_bathing_step_dev.argtypes = [vp, vp, vp, vp, vp, vp]
     lib.ag_bathing_step_host.argtypes = [vp, vp, vp, vp, vp, vp]
+    lib.ag_bathing_set_target_frames.argtypes = [vp, vp, vp]
     lib.ag_cloth_init.argtypes = [vp, C.POINTER(AgClothDesc)]
     lib.ag_cloth_set_state.argtypes = [vp, vp, vp, vp]
     lib.ag_cloth_get_state.argtypes = [vp, vp, vp]
@@ -285,5 +286,5 @@ EXPORTED_SYMBOLS = [
     'ag_cloth_init', 'ag_cloth_set_state', 'ag_cloth_get_state', 'ag_cloth_set_anchor', 'ag_cloth_anchor_follow', 'ag_cloth_set_gravity',
     'ag_cloth_get_contacts', 'ag_cloth_device_state', 'ag_scratch_init', 'ag_scratch_step_dev', 'ag_scratch_step_host', 'ag_render', 'ag_set_body_gravity', 'ag_get_link_aabb', 'ag_dressing_init', 'ag_dressing_reset_episode', 'ag_dressing_set_tremor', 'ag_set_motor_force_scale', 'ag_dressing_step_dev', 'ag_dressing_step_host',
     'ag_overflow_count', 'ag_get_solver_stats', 'ag_get_pgs_cycles', 'ag_get_pgs_trips', 'ag_get_pgs_occupancy', 'ag_profile_enable', 'ag_profile_get',
-    'ag_coop_init', 'ag_coop_step_dev', 'ag_coop_step_host', 'ag_coop_classify',
+    'ag_coop_init', 'ag_coop_step_dev', 'ag_coop_step_host', 'ag_coop_classify', 'ag_bathing_set_target_frames',
 ]

@@ -1,6 +1,8 @@
 // ag_bathing.cuh — fused BedBathingEnv step (reference envs/bed_bathing.py:12-111 + envs/env.py:174-274):
 // action -> PD targets -> frame_skip substeps -> obs[24] / reward / done, with the wiping-target bookkeeping
 // of get_total_force (bed_bathing.py:41-78) as a per-env bit-free mask over the target points.
+// With a controllable person (BedBathingSawyerHuman-v1, run by ag_coop.cuh) the right arm moves, and bathing_track_body
+// re-places every target on its upper-arm / forearm link (update_targets, bed_bathing.py:190-203).
 #pragma once
 #include "ag_device.cuh"
 #include "ag_feeding.cuh"
@@ -10,17 +12,20 @@ struct BathDev {
   AgBathingParams P;
   int *male, *iteration, *task_success, *total_targets;
   float* action;                  // [7][N]
-  float* targets;                 // [T][3][N] world positions (the person is static after reset)
+  float* targets;                 // [T][3][N] world positions (fixed at reset for a static person, re-placed by k_bath_track)
   int* alive;                     // [T][N] 1 = not wiped yet (0 for padding beyond the env's target count)
+  int* target_link;               // [T][N] global link the target rides on, -1 = padding (ag_bathing_set_target_frames)
+  float* target_local;            // [T][3][N] the target in that link's frame
   float* dist_part;               // [human collider slot][N] partial minima of the tool-person distance
   int n_slots;                    // max colliders of a person
 };
 
-// action -> PD targets (env.py:187-217), same accumulate-with-limit-clamp rule as the feeding path
+// action -> PD targets (env.py:187-217), same accumulate-with-limit-clamp rule as the feeding path.
+// p0 = action [N][7 + i0] (env-major; the robot's 7 come first), p1 = BathDev*
 AG_HDN inline void bathing_pre_body(int e, const SimDev& S, const KP& p) {
   const int N = S.N;
   const BathDev& B = *(const BathDev*)p.p1;
-  const float* act = (const float*)p.p0 + (size_t)e * 7;
+  const float* act = (const float*)p.p0 + (size_t)e * (7 + p.i0);
   B.iteration[e] += 1;
   for (int j = 0; j < 7; j++) {
     float raw = act[j];
@@ -62,7 +67,18 @@ AG_HDN inline void bathing_dist_body(int tid, const SimDev& S, const KP& p) {
   B.dist_part[(size_t)slot * N + e] = best;
 }
 
-// obs / reward / done.  p0 = action, p1 = BathDev*, p2 = obs [N][24], p3 = reward, p4 = done, p5 = info [N][4]
+// thread = (target, env): update_targets (bed_bathing.py:190-203) from the current link poses, after the step's final k_fk
+AG_HDN inline void bathing_track_body(int tid, const SimDev& S, const KP& p) {
+  const int N = S.N;
+  const BathDev& B = *(const BathDev*)p.p1;
+  const int e = tid % N, t = tid / N;
+  const int link = B.target_link[(size_t)t * N + e];
+  if (link < 0) return;
+  st3(B.targets, t, N, e, ld3(S.lpos, link, N, e) + qrot(ld4(S.lquat, link, N, e), ld3(B.target_local, t, N, e)));
+}
+
+// obs / reward / done.  p0 = action [N][7 + i0] (the reward's action term covers the whole raw row), p1 = BathDev*, p2 = obs [N][24],
+// p3 = reward, p4 = done, p5 = info [N][4]
 AG_HDN inline void bathing_post_body(int e, const SimDev& S, const KP& p) {
   const int N = S.N;
   const BathDev& B = *(const BathDev*)p.p1;
@@ -130,6 +146,7 @@ AG_HDN inline void bathing_post_body(int e, const SimDev& S, const KP& p) {
   float pref = P.c_v * (-norm(lin)) + P.c_f * (-(total_on_human - tool_on_human)) + P.c_hf * (tool_on_human < 10.f ? 0.f : -tool_on_human);
   float an = 0.f;
   for (int j = 0; j < 7; j++) { float a = B.action[(size_t)j * N + e]; an += a * a; }
+  for (int j = 0; j < p.i0; j++) { float a = ((const float*)p.p0)[(size_t)e * (7 + p.i0) + 7 + j]; an += a * a; }
   ((float*)p.p3)[e] = P.w_distance * (-dmin) + P.w_action * (-sqrtf(an)) + P.w_wiping * (float)new_pts + pref;
   ((float*)p.p4)[e] = B.iteration[e] >= 200 ? 1.f : 0.f;
   float* info = (float*)p.p5 + (size_t)e * 4;

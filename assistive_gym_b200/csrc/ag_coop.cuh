@@ -1,4 +1,5 @@
-// ag_coop.cuh — the person's half of the fused co-optimisation step (FeedingJacoHuman-v1, ScratchItchJacoHuman-v1).
+// ag_coop.cuh — the person's half of the fused co-optimisation step (FeedingJacoHuman-v1, ScratchItchJacoHuman-v1,
+// BedBathingSawyerHuman-v1).
 //
 // Reference semantics restated here:
 //   coop_pre      AssistiveEnv.take_step for the Human agent (envs/env.py:174-222): the human slice of the action, clipped and
@@ -8,9 +9,9 @@
 //                 Human.enforce_realistic_joint_limits (agents/human.py:134-152): the joint-limit MLP classifies the arm pose,
 //                 an unreachable pose is replaced by the env's last reachable one
 //   coop_obs      the person's observation in its own base frame: FeedingEnv._get_obs (feeding.py:101-111, 23 floats),
-//                 ScratchItchEnv._get_obs (scratch_itch.py:75-84, 34 floats)
-// The robot's half, the reward, done and info are the task's own kernels (k_feed_* / k_scratch_*), which read the wider
-// action rows through KP.i0.
+//                 ScratchItchEnv._get_obs (scratch_itch.py:75-84, 34 floats), BedBathingEnv._get_obs (bed_bathing.py:97-105, 28 floats)
+// The robot's half, the reward, done and info are the task's own kernels (k_feed_* / k_scratch_* / k_bath_*), which read the
+// wider action rows through KP.i0.
 //
 // The limit arithmetic and the classifier's input mapping run in fp64, as the per-call path does on the host, so that the
 // clamps, the motor targets and the fp32 classifier inputs are the host's values.  The classifier itself is plain fp32 FMAs
@@ -18,6 +19,7 @@
 #pragma once
 #include <math.h>
 #include "ag_device.cuh"
+#include "ag_bathing.cuh"
 #include "ag_feeding.cuh"
 #include "ag_scratch.cuh"
 #include "../../include/agphys.h"
@@ -146,7 +148,8 @@ AG_HD void coop_base_frame(const SimDev& S, int e, int body, f3& bp, q4& bqi) {
 AG_HD int coop_put3(float* o, int i, f3 v) { o[i] = v.x; o[i + 1] = v.y; o[i + 2] = v.z; return i + 3; }
 AG_HD int coop_put4(float* o, int i, q4 v) { o[i] = v.x; o[i + 1] = v.y; o[i + 2] = v.z; o[i + 3] = v.w; return i + 4; }
 
-// p1 = CoopDev*, p2 = FeedDev* | ScratchDev*, p3 = obs_human [N][23 | 34], p4 = info [N][4] written by the task's post kernel
+// p1 = CoopDev*, p2 = FeedDev* | ScratchDev* | BathDev*, p3 = obs_human [N][23 | 34 | 28], p4 = info [N][4] written by the task's
+// post kernel
 AG_HDN inline void coop_obs_body(int e, const SimDev& S, const KP& p) {
   const int N = S.N;
   const CoopDev& C = *(const CoopDev*)p.p1;
@@ -173,6 +176,18 @@ AG_HDN inline void coop_obs_body(int e, const SimDev& S, const KP& p) {
     i = coop_put3(o, i, qrot(bqi, hp - bp)); i = coop_put4(o, i, qmul(bqi, hq));
     o[i++] = info[2];                         // robot force on the person
     o[i++] = info[3];                         // spoon force on the person
+  } else if (P.task == 2) {                   // bed_bathing.py:97-105
+    const BathDev& B = *(const BathDev*)p.p2;
+    f3 tp = ld3(S.lpos, B.P.cloth_link, N, e); q4 tq = ld4(S.lquat, B.P.cloth_link, N, e);
+    float* o = (float*)p.p3 + (size_t)e * 28;
+    i = coop_put3(o, i, qrot(bqi, tp - bp)); i = coop_put4(o, i, qmul(bqi, tq));
+    for (int c = 0; c < P.n_ctrl; c++) o[i++] = ld1(S.jq, links[P.ctrl[c]], N, e);
+    for (int j = 0; j < 3; j++) {
+      const int k = male ? B.P.arm_points_m[j] : B.P.arm_points_f[j];
+      i = coop_put3(o, i, qrot(bqi, ld3(S.lpos, k, N, e) - bp));
+    }
+    o[i++] = info[0];                         // total force on the person
+    o[i++] = info[2];                         // wiper-cloth force on the person
   } else {                                    // scratch_itch.py:75-84
     const ScratchDev& D = *(const ScratchDev*)p.p2;
     f3 tp = ld3(S.lpos, D.P.tool_tip_link, N, e); q4 tq = ld4(S.lquat, D.P.tool_tip_link, N, e);

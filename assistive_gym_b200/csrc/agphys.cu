@@ -107,6 +107,7 @@ AG_KERNEL(k_ik, ik_body)
 AG_KERNEL(k_bath_pre, bathing_pre_body)
 AG_KERNEL(k_bath_dist, bathing_dist_body)
 AG_KERNEL(k_bath_post, bathing_post_body)
+AG_KERNEL(k_bath_track, bathing_track_body)
 AG_KERNEL(k_dress_pre, dressing_pre_body)
 AG_KERNEL(k_dress_post, dressing_post_body)
 AG_KERNEL(k_scratch_pre, scratch_pre_body)
@@ -176,6 +177,7 @@ struct AgSim {
   // feeding
   FeedDev F; FeedDev* F_dev; bool feeding;
   BathDev B; BathDev* B_dev; bool bathing;
+  bool bath_frames;                    // ag_bathing_set_target_frames since the last ag_bathing_init
   float *h_bpin_in, *h_bpin_out, *d_baction, *d_bobs, *d_breward, *d_bdone, *d_binfo;
   float *d_action, *d_obs, *d_reward, *d_done, *d_info;
   float *h_pin_in, *h_pin_out;
@@ -1673,6 +1675,31 @@ int ag_bathing_init(AgSim* s, const AgBathingParams* p, const int32_t* gender_is
   if (h2d(s, B.iteration, zero.data(), sizeof(int) * N) || h2d(s, B.task_success, zero.data(), sizeof(int) * N)) return -1;
   if (h2d(s, s->B_dev, &s->B, sizeof(BathDev))) return fail("BathDev upload failed");
   s->bathing = true;
+  s->bath_frames = false;
+  return 0;
+}
+int ag_bathing_set_target_frames(AgSim* s, const int32_t* link, const float* local) {
+  DevGuard guard__(s->device);
+  if (!s->bathing) return fail("ag_bathing_set_target_frames: call ag_bathing_init first");
+  if (!link || !local) return fail("ag_bathing_set_target_frames: bad arguments");
+  const int N = s->S.N, T = s->B.P.n_targets_max;
+  BathDev& B = s->B;
+  std::vector<int> lk((size_t)T * N); std::vector<float> lo((size_t)T * 3 * N);
+  for (int e = 0; e < N; e++)
+    for (int t = 0; t < T; t++) {
+      const int k = link[(size_t)e * T + t];
+      if (k != -1 && (k < 0 || k >= s->nl || (s->link_body[k] != B.P.human_body_m && s->link_body[k] != B.P.human_body_f)))
+        return fail("ag_bathing_set_target_frames: bad target link (a link of either person, or -1)");
+      lk[(size_t)t * N + e] = k;
+      for (int c = 0; c < 3; c++) lo[((size_t)t * 3 + c) * N + e] = local[((size_t)e * T + t) * 3 + c];
+    }
+  if (!B.target_link) {
+    B.target_link = dalloc<int>(s, (size_t)T * N); B.target_local = dalloc<float>(s, (size_t)T * 3 * N);
+    if (!B.target_link || !B.target_local) return fail("device allocation failed");
+    if (h2d(s, s->B_dev, &s->B, sizeof(BathDev))) return fail("BathDev upload failed");
+  }
+  if (h2d(s, B.target_link, lk.data(), lk.size() * sizeof(int)) || h2d(s, B.target_local, lo.data(), lo.size() * sizeof(float))) return -1;
+  s->bath_frames = true;
   return 0;
 }
 static int bathing_step_enqueue(AgSim* s, const float* action_dev, float* obs, float* reward, float* done, float* info) {
@@ -1743,7 +1770,11 @@ int ag_coop_init(AgSim* s, const AgCoopParams* p, const double* limit_scale, con
   } else if (p->task == 1) {
     if (!s->scratch) return fail("ag_coop_init: call ag_scratch_init first");
     if (p->n_ctrl != 10) return fail("ag_coop_init: the scratch-itch person has 10 controllable joints");
-  } else return fail("ag_coop_init: task must be 0 (feeding) or 1 (scratch itch)");
+  } else if (p->task == 2) {
+    if (!s->bathing) return fail("ag_coop_init: call ag_bathing_init first");
+    if (!s->bath_frames) return fail("ag_coop_init: call ag_bathing_set_target_frames first");
+    if (p->n_ctrl != 10) return fail("ag_coop_init: the bed-bathing person has 10 controllable joints");
+  } else return fail("ag_coop_init: task must be 0 (feeding), 1 (scratch itch) or 2 (bed bathing)");
   if (p->human_body_m < 0 || p->human_body_m >= s->nb || p->human_body_f < 0 || p->human_body_f >= s->nb) return fail("ag_coop_init: bad body");
   if (p->n_joints < 1 || p->n_joints > AG_COOP_MAXJ) return fail("ag_coop_init: 1..48 joints");
   for (int j = 0; j < p->n_joints; j++) {
@@ -1780,8 +1811,8 @@ int ag_coop_init(AgSim* s, const AgCoopParams* p, const double* limit_scale, con
 #endif
   }
   C.P = *p;
-  C.frame_skip = p->task == 0 ? s->F.P.frame_skip : s->SD.P.frame_skip;
-  C.male = p->task == 0 ? s->F.male : s->SD.male;
+  C.frame_skip = p->task == 0 ? s->F.P.frame_skip : (p->task == 1 ? s->SD.P.frame_skip : s->B.P.frame_skip);
+  C.male = p->task == 0 ? s->F.male : (p->task == 1 ? s->SD.male : s->B.male);
   C.mlp_on = mlp != nullptr;
   std::vector<float> none((size_t)4 * N, nanf(""));
   if (h2d(s, C.limit_scale, sc.data(), sizeof(double) * N) || h2d(s, C.prev_pose, none.data(), sizeof(float) * 4 * N)) return -1;
@@ -1812,11 +1843,10 @@ static void coop_limits_launch(AgSim* s) {
   s->launches++;
 }
 static int coop_step_enqueue(AgSim* s, const float* action_dev, float* obs, float* reward, float* done, float* info) {
-  const int N = s->S.N, k = s->CO.P.n_ctrl;
-  const bool feed = s->CO.P.task == 0;
-  void* task_dev = feed ? (void*)s->F_dev : (void*)s->SD_dev;
+  const int N = s->S.N, k = s->CO.P.n_ctrl, task = s->CO.P.task;
+  void* task_dev = task == 0 ? (void*)s->F_dev : (task == 1 ? (void*)s->SD_dev : (void*)s->B_dev);
   KP p = kp0(); p.p0 = action_dev; p.p1 = task_dev; p.i0 = k;
-  if (feed) LAUNCH(s, k_feed_pre, N, p); else LAUNCH(s, k_scratch_pre, N, p);
+  if (task == 0) LAUNCH(s, k_feed_pre, N, p); else if (task == 1) LAUNCH(s, k_scratch_pre, N, p); else LAUNCH(s, k_bath_pre, N, p);
   KP c = kp0(); c.p0 = action_dev; c.p1 = s->CO_dev;
   LAUNCH(s, k_coop_pre, N, c);
   const int sub = s->cfg.num_substeps > 0 ? s->cfg.num_substeps : 1;
@@ -1827,16 +1857,24 @@ static int coop_step_enqueue(AgSim* s, const float* action_dev, float* obs, floa
   KP z = kp0();
   LAUNCH(s, k_fk, (size_t)s->S.nb * N, z);
   KP q = kp0(); q.p0 = action_dev; q.p1 = task_dev; q.p2 = obs; q.p3 = reward; q.p4 = done; q.p5 = info; q.i0 = k;
-  if (feed) {
+  if (task != 1) {
     KP a = kp0(); a.p0 = s->S.movcol; a.i0 = s->S.nmovcol;
     LAUNCH(s, k_aabb, (size_t)s->S.nmovcol * N, a);
     KP l = kp0(); l.p0 = s->S.movlink; l.i0 = s->S.nmovlink;
     LAUNCH(s, k_linkaabb, (size_t)s->S.nmovlink * N, l);
+  }
+  if (task == 0) {
     KP f = kp0(); f.p1 = s->F_dev;
     LAUNCH(s, k_feed_food, (size_t)N * s->F.P.n_foods, f);
     LAUNCH(s, k_feed_post, N, q);
-  } else {
+  } else if (task == 1) {
     LAUNCH(s, k_scratch_post, N, q);
+  } else {             // the targets follow the arm (update_targets), with k_coop_limits' restorations in the final poses
+    KP t = kp0(); t.p1 = s->B_dev;
+    LAUNCH(s, k_bath_track, (size_t)N * s->B.P.n_targets_max, t);
+    KP d = kp0(); d.p1 = s->B_dev;
+    LAUNCH(s, k_bath_dist, (size_t)N * s->B.n_slots, d);
+    LAUNCH(s, k_bath_post, N, q);
   }
   KP o = kp0(); o.p1 = s->CO_dev; o.p2 = task_dev; o.p3 = s->coop_obs_h; o.p4 = info;
   LAUNCH(s, k_coop_obs, N, o);
@@ -1845,6 +1883,7 @@ static int coop_step_enqueue(AgSim* s, const float* action_dev, float* obs, floa
 int ag_coop_step_dev(AgSim* s, const float* action_dev, float* obs_robot_dev, float* obs_human_dev, float* reward_dev, float* done_dev, float* info_dev) {
   DevGuard guard__(s->device);
   if (!s->coop) return fail("ag_coop_init not called");
+  if (s->CO.P.task == 2 && !s->bath_frames) return fail("ag_coop_step: call ag_bathing_set_target_frames after ag_bathing_init");
   if (obs_human_dev != s->coop_obs_h) { drop_graph(s, 4); s->coop_obs_h = obs_human_dev; }
   int rc = run_step(s, 4, coop_step_enqueue, action_dev, obs_robot_dev, reward_dev, done_dev, info_dev);
 #ifndef AG_CPU_EMU
@@ -1856,7 +1895,8 @@ int ag_coop_step_host(AgSim* s, const float* action, float* obs_robot, float* ob
   DevGuard guard__(s->device);
   if (!s->coop) return fail("ag_coop_init not called");
   const int N = s->S.N;
-  const size_t ro = s->CO.P.task == 0 ? 25 : 30, ho = s->CO.P.task == 0 ? 23 : 34;
+  static const size_t ro_of[3] = {25, 30, 24}, ho_of[3] = {23, 34, 28};
+  const size_t ro = ro_of[s->CO.P.task], ho = ho_of[s->CO.P.task];
   if (h2d(s, s->d_caction, action, sizeof(float) * N * s->coop_width)) return -1;
   if (ag_coop_step_dev(s, s->d_caction, s->d_cobs_r, s->d_cobs_h, s->d_creward, s->d_cdone, s->d_cinfo)) return -1;
   if (d2h(s, obs_robot, s->d_cobs_r, sizeof(float) * N * ro) || d2h(s, obs_human, s->d_cobs_h, sizeof(float) * N * ho) ||

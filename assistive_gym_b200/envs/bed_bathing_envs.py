@@ -12,3 +12,14 @@ class BedBathingSawyerEnv(BedBathingEnv):
     def __init__(self, n_envs=1, device=0, seed=1001, config=None):
         super().__init__(robot=Sawyer(robot_arm), human=Human(human_controllable_joint_indices, controllable=False),
                          n_envs=n_envs, device=device, seed=seed, config=config)
+
+
+class BedBathingSawyerHumanEnv(BedBathingEnv):
+    """`assistive_gym:BedBathingSawyerHuman-v1` (reference envs/bed_bathing_envs.py): robot and person are both agents; `step` takes
+    {'robot': a7, 'human': a10} and returns dict observations (24 and 28 floats) / rewards / dones (RLlib MultiAgentEnv shape,
+    learn.py:41-59).  The person's right arm is driven by its action and kept inside the realistic joint limits; the wiping targets
+    follow the arm.  Per-call API path; `step_fused` is the same step on the device."""
+
+    def __init__(self, n_envs=1, device=0, seed=1001, config=None):
+        super().__init__(robot=Sawyer(robot_arm), human=Human(human_controllable_joint_indices, controllable=True),
+                         n_envs=n_envs, device=device, seed=seed, config=config)

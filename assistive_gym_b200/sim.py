@@ -232,9 +232,16 @@ class BatchSim:
     # ---- fused bed-bathing path
     def bathing_init(self, params, gender_is_male, targets_world, targets_valid):
         g = _i32(np.broadcast_to(np.asarray(gender_is_male, dtype=np.int32), (self.n,)))
-        T = int(params.n_targets_max)
+        T = self._bath_T = int(params.n_targets_max)
         tw = _f32(targets_world, (self.n, T, 3)); tv = _i32(np.ascontiguousarray(targets_valid, dtype=np.int32).reshape(self.n, T))
         self._ck(self.lib.ag_bathing_init(self.h, C.byref(params), _p(g), _p(tw), _p(tv)))
+
+    def bathing_set_target_frames(self, link, local):
+        """link [n, T] global link id each target rides on (-1 = padding), local [n, T, 3] the target in that link's frame; after
+        `bathing_init`.  The fused co-optimisation step re-places the targets from these frames (update_targets)."""
+        T = int(getattr(self, '_bath_T', None) or np.shape(link)[-1])        # before bathing_init the library reports the error
+        lk = _i32(np.broadcast_to(np.asarray(link, dtype=np.int32), (self.n, T)))
+        self._ck(self.lib.ag_bathing_set_target_frames(self.h, _p(lk), _p(_f32(local, (self.n, T, 3)))))
 
     def bathing_step_host(self, action):
         a = _f32(action, (self.n, 7))
@@ -304,11 +311,11 @@ class BatchSim:
     def scratch_step_dev(self, action_ptr, obs_ptr, reward_ptr, done_ptr, info_ptr):
         self._ck(self.lib.ag_scratch_step_dev(self.h, action_ptr, obs_ptr, reward_ptr, done_ptr, info_ptr))
 
-    # ---- fused co-optimisation path (the person's half; call after feeding_init / scratch_init)
+    # ---- fused co-optimisation path (the person's half; call after feeding_init / scratch_init / bathing_init)
     def coop_init(self, params, limit_scale=None, mlp=None):
         """limit_scale [n] or None; mlp: the packed classifier weights (fp32, agphys.h order) or None"""
         self._coop_params = params
-        self._coop_dims = (25, 23) if params.task == 0 else (30, 34)
+        self._coop_dims = {0: (25, 23), 1: (30, 34), 2: (24, 28)}.get(int(params.task), (0, 0))
         ls = None if limit_scale is None else np.ascontiguousarray(np.broadcast_to(np.asarray(limit_scale, dtype=np.float64), (self.n,)))
         w = None if mlp is None else np.ascontiguousarray(mlp, dtype=np.float32)
         self._ck(self.lib.ag_coop_init(self.h, C.byref(params), _p(ls), _p(w)))

@@ -246,6 +246,11 @@ int ag_bathing_init(AgSim* sim, const AgBathingParams* p, const int32_t* gender_
 /* obs [N][24], reward [N], done [N], info [N][4] = total force on person, task success, cloth force on person, new targets */
 int ag_bathing_step_dev(AgSim* sim, const float* action_dev, float* obs_dev, float* reward_dev, float* done_dev, float* info_dev);
 int ag_bathing_step_host(AgSim* sim, const float* action, float* obs, float* reward, float* done, float* info);
+/* the frames the targets ride on, for a person whose right arm moves (BedBathingSawyerHuman-v1, update_targets
+ * bed_bathing.py:190-203): link [N][T] global id of a link of either person (-1 = padding), local [N][T][3] the target in that
+ * link's frame (host).  Call after ag_bathing_init, which every episode's reset calls; the fused co-optimisation step re-places
+ * the targets from these frames after its last substep.  ag_bathing_step_* keep the world positions of ag_bathing_init. */
+int ag_bathing_set_target_frames(AgSim* sim, const int32_t* link, const float* local);
 
 /* --- cloth: p.loadCloth / p.clothParams / p.getSoftBodyData (dressing.py:25,146-154), stepped inside ag_step with the
  * world's numSubSteps (dressing.py:184).  SURVEY.md section 8(a) row D1.  The model restates Bullet's btSoftBody position
@@ -336,7 +341,7 @@ int ag_scratch_init(AgSim* sim, const AgScratchParams* p, const int32_t* gender_
 int ag_scratch_step_dev(AgSim* sim, const float* action_dev, float* obs_dev, float* reward_dev, float* done_dev, float* info_dev);
 int ag_scratch_step_host(AgSim* sim, const float* action, float* obs, float* reward, float* done, float* info);
 
-/* --- fused co-optimisation step (FeedingJacoHuman-v1, ScratchItchJacoHuman-v1; env.py:174-235 with the person as a second
+/* --- fused co-optimisation step (FeedingJacoHuman-v1, ScratchItchJacoHuman-v1, BedBathingSawyerHuman-v1; env.py:174-235 with the person as a second
  * agent): the robot part is the task's own fused step; the person's part applies the human slice of the action to its
  * controllable joints (clip to [-1, 1], x 0.05, 5-fold accumulate inside its limits), and after every stepSimulation
  * clamps every joint of the person to its limits (Human.enforce_joint_limits) and, with the classifier on, keeps the arm
@@ -344,12 +349,13 @@ int ag_scratch_step_host(AgSim* sim, const float* action, float* obs, float* rew
 #define AG_COOP_MAXJ 48
 #define AG_COOP_MAXC 10
 typedef struct AgCoopParams {
-  int32_t task;                 /* 0 = FeedingEnv (after ag_feeding_init), 1 = ScratchItchEnv (after ag_scratch_init) */
+  int32_t task;                 /* 0 = FeedingEnv (after ag_feeding_init), 1 = ScratchItchEnv (after ag_scratch_init),
+                                   2 = BedBathingEnv (after ag_bathing_init and ag_bathing_set_target_frames) */
   int32_t human_body_m, human_body_f;
   int32_t n_joints;             /* every joint of the person: enforce_joint_limits clamps all of them */
   int32_t joint_links_m[AG_COOP_MAXJ], joint_links_f[AG_COOP_MAXJ];   /* global link ids per gender */
   double  joint_lower[AG_COOP_MAXJ], joint_upper[AG_COOP_MAXJ];       /* template limits (the `limits` impairment scales them) */
-  int32_t n_ctrl;               /* controllable joints = width of the human part of the action: 4 for feeding, 10 for scratch */
+  int32_t n_ctrl;               /* controllable joints = width of the human part of the action: 4 for feeding, 10 for scratch and bathing */
   int32_t ctrl[AG_COOP_MAXC];   /* indices into the joint list */
   float   motor_gain, motor_force;            /* Human.motor_gains / motor_forces: what take_step's control() sets */
   int32_t mlp_slots[4];         /* joint-list indices of shoulder x, y, z and elbow (classifier inputs) */
@@ -361,7 +367,7 @@ typedef struct AgCoopParams {
  * NULL (classifier off).  Resets the per-env last reachable arm pose to "none yet" and sets the person's controllable motors
  * to motor_gain / motor_force (kd 1) in both genders. */
 int ag_coop_init(AgSim* sim, const AgCoopParams* p, const double* limit_scale, const float* mlp);
-/* action [N][7 + n_ctrl] (robot, then person); obs_robot [N][25 | 30], obs_human [N][23 | 34], reward [N], done [N],
+/* action [N][7 + n_ctrl] (robot, then person); obs_robot [N][25 | 30 | 24], obs_human [N][23 | 34 | 28], reward [N], done [N],
  * info [N][4] as the task's own step reports them */
 int ag_coop_step_dev(AgSim* sim, const float* action_dev, float* obs_robot_dev, float* obs_human_dev, float* reward_dev, float* done_dev, float* info_dev);
 int ag_coop_step_host(AgSim* sim, const float* action, float* obs_robot, float* obs_human, float* reward, float* done, float* info);

@@ -1,12 +1,13 @@
-"""Throughput of the co-optimisation envs (FeedingJacoHuman-v1, ScratchItchJacoHuman-v1) on one GPU: the fused device step
+"""Throughput of the co-optimisation envs (FeedingJacoHuman-v1, ScratchItchJacoHuman-v1, BedBathingSawyerHuman-v1) on one GPU: the fused device step
 (`step_fused` / ag_coop_step_dev, graph-replayed) against the per-call `step` (take_step + _get_obs through the C ABI, with the
 host round trips of enforce_joint_limits / the realistic-arm-limit classifier after every substep), at the same batch size.
 
 Prints one JSON line per id: fused env-steps/s (CUDA events around the timed steps after warm-up), per-call env-steps/s (a host
 clock around fewer steps, each of which ends in device-to-host reads), k_coop_limits ms per launch (ag_profile_get, in a
-separate profiled run of the fused step) and the card's name and power limit, read in the same run.
+separate profiled run of the fused step; for BedBathing also k_bath_track, which re-places the wiping targets on the moving arm)
+and the card's name and power limit, read in the same run.
 
-    python tools/gpu_coop_bench.py --n 4096 --steps 50 --warmup 5 --percall-steps 3 [--out profiles/h100_coop_bench.jsonl]
+    python tools/gpu_coop_bench.py --n 4096 --steps 50 --warmup 5 --percall-steps 3 [--ids BedBathingSawyerHuman-v1] [--out profiles/h100_coop_bench.jsonl]
 """
 import argparse
 import json
@@ -69,6 +70,10 @@ def bench(env_id, n, steps, warmup, percall_steps, seed=1001):
     sim.profile_enable(False)
     lim_ms, lim_n = prof.get('k_coop_limits', (0.0, 0))
     pgs_ms, pgs_n = prof.get('k_pgs', (0.0, 0))
+    track = {}
+    if 'k_bath_track' in prof:
+        tr_ms, tr_n = prof['k_bath_track']
+        track = dict(k_bath_track_ms_per_launch=round(tr_ms / max(tr_n, 1), 4), k_bath_track_launches_per_step=tr_n // 3)
     env.close()
     # the per-call path from the same kind of start state (a fresh reset), fewer steps; should it fail at this batch size, it is
     # measured at 1024 envs and the line says so (`percall_n_envs`, `percall_note`)
@@ -83,7 +88,7 @@ def bench(env_id, n, steps, warmup, percall_steps, seed=1001):
                 percall_env_steps_per_s=round(percall_n / percall_s, 1), percall_ms_per_step=round(percall_s * 1e3, 1), percall_steps_timed=percall_steps,
                 fused_over_percall_env_steps=round((n / (fused_ms * 1e-3)) / (percall_n / percall_s), 1),
                 k_coop_limits_ms_per_launch=round(lim_ms / max(lim_n, 1), 4), k_coop_limits_launches_per_step=lim_n // 3,
-                k_pgs_ms_per_launch=round(pgs_ms / max(pgs_n, 1), 4), reset_s=round(reset_s, 2))
+                k_pgs_ms_per_launch=round(pgs_ms / max(pgs_n, 1), 4), reset_s=round(reset_s, 2), **track)
 
 
 def percall(env_id, n, k, steps, seed):
