@@ -1,5 +1,5 @@
 // ag_coop.cuh — the person's half of the fused co-optimisation step (FeedingJacoHuman-v1, ScratchItchJacoHuman-v1,
-// BedBathingSawyerHuman-v1).
+// BedBathingSawyerHuman-v1, DressingPR2Human-v1).
 //
 // Reference semantics restated here:
 //   coop_pre      AssistiveEnv.take_step for the Human agent (envs/env.py:174-222): the human slice of the action, clipped and
@@ -9,9 +9,10 @@
 //                 Human.enforce_realistic_joint_limits (agents/human.py:134-152): the joint-limit MLP classifies the arm pose,
 //                 an unreachable pose is replaced by the env's last reachable one
 //   coop_obs      the person's observation in its own base frame: FeedingEnv._get_obs (feeding.py:101-111, 23 floats),
-//                 ScratchItchEnv._get_obs (scratch_itch.py:75-84, 34 floats), BedBathingEnv._get_obs (bed_bathing.py:97-105, 28 floats)
-// The robot's half, the reward, done and info are the task's own kernels (k_feed_* / k_scratch_* / k_bath_*), which read the
-// wider action rows through KP.i0.
+//                 ScratchItchEnv._get_obs (scratch_itch.py:75-84, 34 floats), BedBathingEnv._get_obs (bed_bathing.py:97-105, 28 floats),
+//                 DressingEnv._get_obs (dressing.py:96-105, 28 floats)
+// The robot's half, the reward, done and info are the task's own kernels (k_feed_* / k_scratch_* / k_bath_* / k_dress_*), which
+// read the wider action rows through KP.i0.
 //
 // The limit arithmetic and the classifier's input mapping run in fp64, as the per-call path does on the host, so that the
 // clamps, the motor targets and the fp32 classifier inputs are the host's values.  The classifier itself is plain fp32 FMAs
@@ -20,6 +21,7 @@
 #include <math.h>
 #include "ag_device.cuh"
 #include "ag_bathing.cuh"
+#include "ag_dressing.cuh"
 #include "ag_feeding.cuh"
 #include "ag_scratch.cuh"
 #include "../../include/agphys.h"
@@ -148,8 +150,8 @@ AG_HD void coop_base_frame(const SimDev& S, int e, int body, f3& bp, q4& bqi) {
 AG_HD int coop_put3(float* o, int i, f3 v) { o[i] = v.x; o[i + 1] = v.y; o[i + 2] = v.z; return i + 3; }
 AG_HD int coop_put4(float* o, int i, q4 v) { o[i] = v.x; o[i + 1] = v.y; o[i + 2] = v.z; o[i + 3] = v.w; return i + 4; }
 
-// p1 = CoopDev*, p2 = FeedDev* | ScratchDev* | BathDev*, p3 = obs_human [N][23 | 34 | 28], p4 = info [N][4] written by the task's
-// post kernel
+// p1 = CoopDev*, p2 = FeedDev* | ScratchDev* | BathDev* | DressPost*, p3 = obs_human [N][23 | 34 | 28 | 28], p4 = info [N][4]
+// written by the task's post kernel
 AG_HDN inline void coop_obs_body(int e, const SimDev& S, const KP& p) {
   const int N = S.N;
   const CoopDev& C = *(const CoopDev*)p.p1;
@@ -188,6 +190,18 @@ AG_HDN inline void coop_obs_body(int e, const SimDev& S, const KP& p) {
     }
     o[i++] = info[0];                         // total force on the person
     o[i++] = info[2];                         // wiper-cloth force on the person
+  } else if (P.task == 3) {                   // dressing.py:96-105
+    const DressDev& D = ((const DressPost*)p.p2)->D;
+    f3 ep = ld3(S.lpos, D.P.ee_link, N, e); q4 eq = ld4(S.lquat, D.P.ee_link, N, e);
+    float* o = (float*)p.p3 + (size_t)e * 28;
+    i = coop_put3(o, i, qrot(bqi, ep - bp)); i = coop_put4(o, i, qmul(bqi, eq));
+    for (int c = 0; c < P.n_ctrl; c++) o[i++] = ld1(S.jq, links[P.ctrl[c]], N, e);
+    for (int j = 0; j < 3; j++) {
+      const int k = male ? D.P.arm_points_m[j] : D.P.arm_points_f[j];
+      i = coop_put3(o, i, qrot(bqi, ld3(S.lpos, k, N, e) - bp));
+    }
+    o[i++] = D.person_force[e];               // cloth force sum (k_dress_post)
+    o[i++] = D.person_force[(size_t)N + e];   // robot force on the person
   } else {                                    // scratch_itch.py:75-84
     const ScratchDev& D = *(const ScratchDev*)p.p2;
     f3 tp = ld3(S.lpos, D.P.tool_tip_link, N, e); q4 tq = ld4(S.lquat, D.P.tool_tip_link, N, e);

@@ -1,6 +1,9 @@
 // ag_dressing.cuh — fused DressingEnv step (reference envs/dressing.py:12-106 + envs/env.py:174-274 + envs/util.py:125-202):
 // action -> PD targets -> frame_skip x (numSubSteps rigid substeps + one cloth launch + anchor follows the end effector)
 // -> sleeve-on-arm reward, cloth forces on the person, obs[24] / reward / done.
+// With a controllable person (DressingPR2Human-v1, run by ag_coop.cuh) the left arm is a second agent; the pre / post kernels
+// then read action rows of 7 + KP.i0 floats, and the post kernel leaves the two forces of the person's observation in
+// `person_force` for k_coop_obs.
 #pragma once
 #include "ag_device.cuh"
 #include "ag_feeding.cuh"
@@ -14,13 +17,15 @@ struct DressDev {
   float* action;                  // [7][N]
   int* tremor_on;                 // [N] the person's impairment is 'tremor' (human.py:80-92)
   float *tremor_rest, *tremor_amp; // [10][N] target_joint_angles of the left arm joints and the tremor amplitudes
+  float* person_force;            // [2][N] cloth force sum and robot force on the person (dressing.py:91-93), for k_coop_obs
 };
 
-// action -> PD targets of the robot's 7 arm joints (env.py:187-217)
+// action -> PD targets of the robot's 7 arm joints (env.py:187-217).
+// p0 = action [N][7 + i0] (env-major; the robot's 7 come first), p1 = DressPost* (its leading DressDev)
 AG_HDN inline void dressing_pre_body(int e, const SimDev& S, const KP& p) {
   const int N = S.N;
   const DressDev& D = *(const DressDev*)p.p1;
-  const float* act = (const float*)p.p0 + (size_t)e * 7;
+  const float* act = (const float*)p.p0 + (size_t)e * (7 + p.i0);
   D.iteration[e] += 1;
   for (int j = 0; j < 7; j++) {
     float raw = act[j];
@@ -67,7 +72,7 @@ AG_HD bool dress_points_around(const f3* pts, f3 normal, f3 origin) {
   return ta && tb && ba && bb;
 }
 
-// obs / reward / done.  p0 = action, p1 = DressPost* (the fused step's state + the cloth it reads), p2 = obs [N][24],
+// obs / reward / done.  p0 = action [N][7 + i0] (the reward's action term covers the whole raw row), p1 = DressPost* (the fused step's state + the cloth it reads), p2 = obs [N][24],
 // p3 = reward, p4 = done, p5 = info [N][4] = total force on the person, task success, reward_dressing, sleeve state
 // (1: forearm in the sleeve, 2: upper arm, 3: both)
 struct DressPost { DressDev D; const ClothDev* C; };
@@ -149,6 +154,7 @@ AG_HDN inline void dressing_post_body(int e, const SimDev& S, const KP& p) {
   float pref = P.c_v * (-norm(lin)) + P.c_d * (-cloth_sum);          // env.py:237-274 with the dressing arguments
   float an = 0.f;
   for (int j = 0; j < 7; j++) { float a = D.action[(size_t)j * N + e]; an += a * a; }
+  for (int j = 0; j < p.i0; j++) { float a = ((const float*)p.p0)[(size_t)e * (7 + p.i0) + 7 + j]; an += a * a; }
   ((float*)p.p3)[e] = P.w_dressing * reward_dressing + P.w_action * (-sqrtf(an)) + pref;
   float best = D.task_success[e];
   if (reward_dressing > best) { best = reward_dressing; D.task_success[e] = best; }
@@ -156,4 +162,5 @@ AG_HDN inline void dressing_post_body(int e, const SimDev& S, const KP& p) {
   float* info = (float*)p.p5 + (size_t)e * 4;
   info[0] = robot_on_human + cloth_sum; info[1] = best >= P.task_success_threshold ? 1.f : 0.f; info[2] = reward_dressing;
   info[3] = (forearm_in ? 1.f : 0.f) + (upperarm_in ? 2.f : 0.f);
+  D.person_force[e] = cloth_sum; D.person_force[(size_t)N + e] = robot_on_human;
 }

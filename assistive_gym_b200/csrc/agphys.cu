@@ -1194,7 +1194,7 @@ int ag_cloth_init(AgSim* s, const AgClothDesc* d) {
   if (s->cloth_npt == 4) { CK(cudaFuncSetAttribute(k_cloth<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); CK(cudaFuncSetAttribute(k_cloth<4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); }
   else { CK(cudaFuncSetAttribute(k_cloth<8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); CK(cudaFuncSetAttribute(k_cloth<8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); }
 #endif
-  drop_graph(s, 0); drop_graph(s, 1); drop_graph(s, 2);
+  drop_graph(s, 0); drop_graph(s, 1); drop_graph(s, 2); drop_graph(s, 4);
   s->cloth = true; s->cloth_sub = 0;
   return 0;
 }
@@ -1250,7 +1250,8 @@ int ag_cloth_set_gravity(AgSim* s, const double g[3]) {
   DevGuard guard__(s->device);
   if (!s->cloth) return fail("ag_cloth_init not called");
   s->C.gx = (float)g[0]; s->C.gy = (float)g[1]; s->C.gz = (float)g[2];
-  drop_graph(s, 0); drop_graph(s, 1); drop_graph(s, 2);   // k_cloth takes ClothDev by value: a captured step holds the old gravity
+  // k_cloth takes ClothDev by value: a captured step (the fused steps and the co-optimisation step) holds the old gravity
+  drop_graph(s, 0); drop_graph(s, 1); drop_graph(s, 2); drop_graph(s, 4);
   return cloth_refresh(s);
 }
 int ag_cloth_get_contacts(AgSim* s, int max_pts, int32_t* count, int32_t* node, float* pos, float* force, int32_t* link) {
@@ -1300,14 +1301,15 @@ int ag_dressing_init(AgSim* s, const AgDressingParams* p, const int32_t* gender_
   if (p->ee_link < 0 || p->ee_link >= s->nl) return fail("ag_dressing_init: bad end effector link");
   DressDev& D = s->DP.D;
   D.P = *p;
-  drop_graph(s, 2);
+  drop_graph(s, 2); drop_graph(s, 4);     // the Dressing co-optimisation step captures ee_link and frame_skip as well
   if (!s->dressing) {
     D.male = dalloc<int>(s, N); D.iteration = dalloc<int>(s, N); D.task_success = dalloc<float>(s, N); D.action = dalloc<float>(s, (size_t)N * 7);
     D.tremor_on = dalloc<int>(s, N); D.tremor_rest = dalloc<float>(s, (size_t)N * 10); D.tremor_amp = dalloc<float>(s, (size_t)N * 10);
+    D.person_force = dalloc<float>(s, (size_t)N * 2);
     s->d_daction = dalloc<float>(s, (size_t)N * 7); s->d_dobs = dalloc<float>(s, (size_t)N * 24);
     s->d_dreward = dalloc<float>(s, N); s->d_ddone = dalloc<float>(s, N); s->d_dinfo = dalloc<float>(s, (size_t)N * 4);
     s->DP_dev = dalloc<DressPost>(s, 1);
-    if (!s->d_dinfo || !s->DP_dev) return fail("device allocation failed");
+    if (!s->d_dinfo || !s->DP_dev || !D.person_force) return fail("device allocation failed");
 #ifndef AG_CPU_EMU
     CK(cudaMallocHost((void**)&s->h_dpin_in, sizeof(float) * N * 7));
     CK(cudaMallocHost((void**)&s->h_dpin_out, sizeof(float) * N * 30));
@@ -1774,7 +1776,10 @@ int ag_coop_init(AgSim* s, const AgCoopParams* p, const double* limit_scale, con
     if (!s->bathing) return fail("ag_coop_init: call ag_bathing_init first");
     if (!s->bath_frames) return fail("ag_coop_init: call ag_bathing_set_target_frames first");
     if (p->n_ctrl != 10) return fail("ag_coop_init: the bed-bathing person has 10 controllable joints");
-  } else return fail("ag_coop_init: task must be 0 (feeding), 1 (scratch itch) or 2 (bed bathing)");
+  } else if (p->task == 3) {
+    if (!s->dressing) return fail("ag_coop_init: call ag_dressing_init first");
+    if (p->n_ctrl != 10) return fail("ag_coop_init: the dressing person has 10 controllable joints");
+  } else return fail("ag_coop_init: task must be 0 (feeding), 1 (scratch itch), 2 (bed bathing) or 3 (dressing)");
   if (p->human_body_m < 0 || p->human_body_m >= s->nb || p->human_body_f < 0 || p->human_body_f >= s->nb) return fail("ag_coop_init: bad body");
   if (p->n_joints < 1 || p->n_joints > AG_COOP_MAXJ) return fail("ag_coop_init: 1..48 joints");
   for (int j = 0; j < p->n_joints; j++) {
@@ -1811,8 +1816,8 @@ int ag_coop_init(AgSim* s, const AgCoopParams* p, const double* limit_scale, con
 #endif
   }
   C.P = *p;
-  C.frame_skip = p->task == 0 ? s->F.P.frame_skip : (p->task == 1 ? s->SD.P.frame_skip : s->B.P.frame_skip);
-  C.male = p->task == 0 ? s->F.male : (p->task == 1 ? s->SD.male : s->B.male);
+  C.frame_skip = p->task == 0 ? s->F.P.frame_skip : (p->task == 1 ? s->SD.P.frame_skip : (p->task == 2 ? s->B.P.frame_skip : s->DP.D.P.frame_skip));
+  C.male = p->task == 0 ? s->F.male : (p->task == 1 ? s->SD.male : (p->task == 2 ? s->B.male : s->DP.D.male));
   C.mlp_on = mlp != nullptr;
   std::vector<float> none((size_t)4 * N, nanf(""));
   if (h2d(s, C.limit_scale, sc.data(), sizeof(double) * N) || h2d(s, C.prev_pose, none.data(), sizeof(float) * 4 * N)) return -1;
@@ -1844,20 +1849,27 @@ static void coop_limits_launch(AgSim* s) {
 }
 static int coop_step_enqueue(AgSim* s, const float* action_dev, float* obs, float* reward, float* done, float* info) {
   const int N = s->S.N, k = s->CO.P.n_ctrl, task = s->CO.P.task;
-  void* task_dev = task == 0 ? (void*)s->F_dev : (task == 1 ? (void*)s->SD_dev : (void*)s->B_dev);
+  void* const task_devs[4] = {s->F_dev, s->SD_dev, s->B_dev, s->DP_dev};
+  void* task_dev = task_devs[task];
   KP p = kp0(); p.p0 = action_dev; p.p1 = task_dev; p.i0 = k;
-  if (task == 0) LAUNCH(s, k_feed_pre, N, p); else if (task == 1) LAUNCH(s, k_scratch_pre, N, p); else LAUNCH(s, k_bath_pre, N, p);
+  if (task == 0) LAUNCH(s, k_feed_pre, N, p); else if (task == 1) LAUNCH(s, k_scratch_pre, N, p);
+  else if (task == 2) LAUNCH(s, k_bath_pre, N, p); else LAUNCH(s, k_dress_pre, N, p);
   KP c = kp0(); c.p0 = action_dev; c.p1 = s->CO_dev;
   LAUNCH(s, k_coop_pre, N, c);
   const int sub = s->cfg.num_substeps > 0 ? s->cfg.num_substeps : 1;
-  for (int f = 0; f < s->CO.frame_skip; f++) {         // stepSimulation, then the person's limits (env.py:223-231)
-    for (int i = 0; i < sub; i++) substep(s);
-    coop_limits_launch(s);
-  }
   KP z = kp0();
-  LAUNCH(s, k_fk, (size_t)s->S.nb * N, z);
+  for (int f = 0; f < s->CO.frame_skip; f++) {         // stepSimulation, then the person's limits (env.py:223-231)
+    for (int i = 0; i < sub; i++) substep(s);          // with a cloth, the last one launches k_cloth
+    coop_limits_launch(s);
+    if (task == 3) {     // then update_targets (dressing.py:210): the gown's anchor goes to the end effector
+      LAUNCH(s, k_fk, (size_t)s->S.nb * N, z);         // k_coop_limits' restored poses are what the next cloth snapshot sees
+      KP a = kp0(); a.p0 = s->C_dev; a.i0 = s->DP.D.P.ee_link;
+      LAUNCH(s, k_cloth_follow, N, a);
+    }
+  }
+  if (task != 3) LAUNCH(s, k_fk, (size_t)s->S.nb * N, z);
   KP q = kp0(); q.p0 = action_dev; q.p1 = task_dev; q.p2 = obs; q.p3 = reward; q.p4 = done; q.p5 = info; q.i0 = k;
-  if (task != 1) {
+  if (task == 0 || task == 2) {
     KP a = kp0(); a.p0 = s->S.movcol; a.i0 = s->S.nmovcol;
     LAUNCH(s, k_aabb, (size_t)s->S.nmovcol * N, a);
     KP l = kp0(); l.p0 = s->S.movlink; l.i0 = s->S.nmovlink;
@@ -1869,6 +1881,8 @@ static int coop_step_enqueue(AgSim* s, const float* action_dev, float* obs, floa
     LAUNCH(s, k_feed_post, N, q);
   } else if (task == 1) {
     LAUNCH(s, k_scratch_post, N, q);
+  } else if (task == 3) {
+    LAUNCH(s, k_dress_post, N, q);
   } else {             // the targets follow the arm (update_targets), with k_coop_limits' restorations in the final poses
     KP t = kp0(); t.p1 = s->B_dev;
     LAUNCH(s, k_bath_track, (size_t)N * s->B.P.n_targets_max, t);
@@ -1884,6 +1898,7 @@ int ag_coop_step_dev(AgSim* s, const float* action_dev, float* obs_robot_dev, fl
   DevGuard guard__(s->device);
   if (!s->coop) return fail("ag_coop_init not called");
   if (s->CO.P.task == 2 && !s->bath_frames) return fail("ag_coop_step: call ag_bathing_set_target_frames after ag_bathing_init");
+  if (s->CO.P.task == 3 && s->cloth_sub != 0) return fail("ag_coop_step: a stepSimulation is half done (ag_step with a partial substep count?)");
   if (obs_human_dev != s->coop_obs_h) { drop_graph(s, 4); s->coop_obs_h = obs_human_dev; }
   int rc = run_step(s, 4, coop_step_enqueue, action_dev, obs_robot_dev, reward_dev, done_dev, info_dev);
 #ifndef AG_CPU_EMU
@@ -1895,7 +1910,7 @@ int ag_coop_step_host(AgSim* s, const float* action, float* obs_robot, float* ob
   DevGuard guard__(s->device);
   if (!s->coop) return fail("ag_coop_init not called");
   const int N = s->S.N;
-  static const size_t ro_of[3] = {25, 30, 24}, ho_of[3] = {23, 34, 28};
+  static const size_t ro_of[4] = {25, 30, 24, 24}, ho_of[4] = {23, 34, 28, 28};
   const size_t ro = ro_of[s->CO.P.task], ho = ho_of[s->CO.P.task];
   if (h2d(s, s->d_caction, action, sizeof(float) * N * s->coop_width)) return -1;
   if (ag_coop_step_dev(s, s->d_caction, s->d_cobs_r, s->d_cobs_h, s->d_creward, s->d_cdone, s->d_cinfo)) return -1;

@@ -14,11 +14,19 @@ Differences forced by lock-step batching / the 32-DoF budget of one env (DESIGN.
     data here, so it is drawn but has no effect; `weakness` (per-env motor force scale) and `tremor` are simulated;
   * a tremor person is clamped to its joint limits after every stepSimulation (env.py:226-229); the clamp flag is per joint,
     not per env, so it is on for the arm joints of every env (the limit rows keep non-tremor arms inside anyway).
+
+With `controllable_person=True` (DressingPR2Human-v1) the person's left arm is a second agent.  The template is the same (the left
+arm already keeps its mass); the impairment is drawn with 'no_tremor' (feeding.py:59 does the same for its co-optimisation id);
+`limits` acts through the per-env scaled clamps of the co-optimisation kernels and clips the start pose; `weakness` is drawn but
+does not act, because a controllable person gets no reactive force (dressing.py:124).  While the gown settles the arm is held
+with gain 0.05 and force 1 (dressing.py:142-144), and no per-substep hard clamp is set on it: the reference clamps the person
+once per stepSimulation (env.py:226-231), as `k_coop_limits` does.
 """
 import numpy as np
 
 from . import capi
 from .cloth import ClothModel
+from .feeding_batch import coop_params, pack_mlp
 from .human_model import create_human
 from .kinematics import BodyKinematics, q_axis, q_from_rpy, q_mul, q_rot
 from .toc import jlwki, position_robot_toc  # noqa: F401
@@ -32,6 +40,7 @@ PR2 = dict(arm=[64, 65, 66, 68, 69, 71, 72], ee=76, gripper=[79, 80, 81, 82], gr
            toc_base_pos_offset=[1.7, 0.7, 0], ee_orient_rpy=[0, 0, np.pi], ee_orient_shoulder_rpy=[0, 0, np.pi * 3 / 2.0])
 LEFT_ARM_JOINTS = list(range(10, 20))                       # human.left_arm_joints (dressing_envs.py)
 L_SHOULDER, L_ELBOW, L_WRIST = 15, 17, 19                   # human.py:26-28
+L_ARM_LIMIT_JOINTS = [13, 14, 15, 16]                       # left shoulder x, y, z and elbow: the classifier's inputs (human.py:137-140)
 # degrees (dressing.py:120): right elbow, left shoulder x, left elbow, hips, knees
 HUMAN_PRESET = {6: -90, 13: -45, 16: -90, 28: -90, 31: 80, 35: -90, 38: 80}
 RADII = {'male': (0.043, 0.043, 0.043), 'female': (0.0355, 0.0355, 0.0355)}     # hand, elbow, shoulder (human_creation.py:89,140)
@@ -42,8 +51,41 @@ CLOTH_POSITION = np.array([0.02, -0.38, 0.84])              # dressing.py:146 (s
 CLOTH_SCALE = 1.4
 
 
+def sleeve_on_arm_reward(triangle1_points, triangle2_points, shoulder_pos, elbow_pos, wrist_pos, hand_radius, elbow_radius, shoulder_radius):
+    """Util.sleeve_on_arm_reward (util.py:125-202) for one env, in fp64: (forearm_in_sleeve, upperarm_in_sleeve,
+    distance_along_forearm, distance_along_upperarm, distance_to_hand, distance_to_elbow, distance_to_shoulder, forearm_length,
+    upperarm_length).  The per-call co-optimisation step computes its reward with it; `dressing_post_body` is the fused twin."""
+    def signed_volume(a, b, c, d):
+        return (1.0 / 6.0) * np.dot(np.cross(b - a, c - a), d - a)
+
+    def line_hits_triangle(p0, p1, p2, q0, q1):
+        if np.sign(signed_volume(q0, p0, p1, p2)) != np.sign(signed_volume(q1, p0, p1, p2)):
+            return np.sign(signed_volume(q0, q1, p0, p1)) == np.sign(signed_volume(q0, q1, p1, p2)) == np.sign(signed_volume(q0, q1, p2, p0))
+        return False
+
+    def points_around(pts, normal, origin):
+        t = np.cross(np.array([1.0, 1.0, 0.0]), normal); t = t / np.linalg.norm(t)
+        b = np.cross(t, normal); b = b / np.linalg.norm(b)
+        dt, db = (pts - origin) @ t, (pts - origin) @ b
+        return bool(np.any(dt > 0) and np.any(dt < 0) and np.any(db > 0) and np.any(db < 0))
+    t1, t2 = np.asarray(triangle1_points, dtype=np.float64), np.asarray(triangle2_points, dtype=np.float64)
+    sh, el, wr = (np.asarray(v, dtype=np.float64) for v in (shoulder_pos, elbow_pos, wrist_pos))
+    hand_end = wr + (wr - el) / np.linalg.norm(wr - el) * hand_radius * 2
+    elbow_end = el + (el - wr) / np.linalg.norm(wr - el) * elbow_radius
+    shoulder_end = sh + (sh - el) / np.linalg.norm(sh - el) * shoulder_radius
+    pts = np.concatenate([t1, t2], axis=0)
+    nf = (hand_end - elbow_end) / np.linalg.norm(hand_end - elbow_end)
+    nu = (elbow_end - shoulder_end) / np.linalg.norm(elbow_end - shoulder_end)
+    forearm_in = points_around(pts, nf, hand_end) and (line_hits_triangle(*t1, hand_end, elbow_end) or line_hits_triangle(*t2, hand_end, elbow_end))
+    upperarm_in = points_around(pts, nu, shoulder_end) and (line_hits_triangle(*t1, elbow_end, shoulder_end) or line_hits_triangle(*t2, elbow_end, shoulder_end))
+    centre = pts.mean(axis=0)
+    return (forearm_in, upperarm_in, np.linalg.norm(centre - hand_end), np.linalg.norm(centre - el), np.linalg.norm(hand_end - centre),
+            np.linalg.norm(elbow_end - centre), np.linalg.norm(shoulder_end - centre), np.linalg.norm(hand_end - elbow_end), np.linalg.norm(el - sh))
+
+
 class DressingBatch:
-    def __init__(self):
+    def __init__(self, controllable_person=False):
+        self.controllable_person = bool(controllable_person)
         b = SceneBuilder()
         self.builder = b
         b.set_gravity([0, 0, -9.81])
@@ -137,16 +179,22 @@ class DressingBatch:
         return P
 
     # ------------------------------------------------------------------ batched reset
-    def sample(self, n, rng, impairment='random'):
-        """impairment: 'random' (human.py:80-81), 'no_tremor', or one of none / limits / weakness / tremor."""
+    def sample(self, n, rng, impairment=None):
+        """impairment: 'random' (human.py:80-81), 'no_tremor', or one of none / limits / weakness / tremor; by default 'random', and
+        'no_tremor' for a controllable person.  A controllable person's `limit_scale` is drawn after every other field."""
+        if impairment is None:
+            impairment = 'no_tremor' if self.controllable_person else 'random'
         names = ('none', 'limits', 'weakness', 'tremor')
         imp = rng.integers(0, 4, size=n) if impairment == 'random' else (rng.integers(0, 3, size=n) if impairment == 'no_tremor' else np.full(n, names.index(impairment)))
-        return dict(plane_friction=rng.uniform(0.025, 0.5, size=n),                  # env.py:120
+        s = dict(plane_friction=rng.uniform(0.025, 0.5, size=n),                  # env.py:120
                     male=rng.integers(0, 2, size=n).astype(np.int32),                # human.py:76-77
                     impairment=imp.astype(np.int32),
                     strength=np.where(imp == 2, rng.uniform(0.25, 1.0, size=n), 1.0),                                       # human.py:86
                     tremors=np.where((imp == 3)[:, None], rng.uniform(np.deg2rad(-10), np.deg2rad(10), size=(n, 10)), 0.0),   # human.py:92
                     ee_offset=rng.uniform(-0.05, 0.05, size=(n, 3)))                 # dressing.py:129
+        if self.controllable_person:
+            s['limit_scale'] = np.where(imp == 1, rng.uniform(0.5, 1.0, size=n), 1.0)                                        # human.py:85
+        return s
 
     def human_pose(self):
         out = {}
@@ -178,13 +226,21 @@ class DressingBatch:
         for g, hb in self.humans.items():
             links, q = self.human_pose()[g]
             qn = np.tile(q, (n, 1))
+            if self.controllable_person:     # enforce_joint_limits at the `limits` impairment's scaled limits (human.py:121)
+                lo, hi = self.person_limits(links)
+                sc_ = np.asarray(s.get('limit_scale', np.ones(n)), dtype=np.float64)[:, None]
+                qn = np.clip(qn, lo[None] * sc_, hi[None] * sc_)
             sim.set_joint_state(links, q=qn, qd=np.zeros_like(qn))
             sim.set_body_active(hb, np.where(male if g == 'male' else ~male, 1, 0).astype(np.int32))
             al = self.human_arm_links[g]
-            tgt = np.tile(q[LEFT_ARM_JOINTS], (n, 1))
-            sim.set_motor(al, MOTOR_POSITION, target=tgt, kp=[0.01] * 10, kd=[1.0] * 10, max_force=[1.0] * 10)
-            sim.set_motor_force_scale(al, np.repeat(s.get('strength', np.ones(n))[:, None], 10, axis=1))                    # forces = 1 * strength (human.py:126)
-            sim.set_hard_limits(al, True)
+            tgt = qn[:, LEFT_ARM_JOINTS]
+            if self.controllable_person:     # held while the gown settles (dressing.py:142-144); no reactive force, no strength
+                sim.set_motor(al, MOTOR_POSITION, target=tgt, kp=[0.05] * 10, kd=[1.0] * 10, max_force=[1.0] * 10)
+                sim.set_motor_force_scale(al, np.ones((n, 10)))
+            else:
+                sim.set_motor(al, MOTOR_POSITION, target=tgt, kp=[0.01] * 10, kd=[1.0] * 10, max_force=[1.0] * 10)
+                sim.set_motor_force_scale(al, np.repeat(s.get('strength', np.ones(n))[:, None], 10, axis=1))                # forces = 1 * strength (human.py:126)
+                sim.set_hard_limits(al, True)
         self.human_rest = np.tile(self.human_pose()['male'][1][LEFT_ARM_JOINTS], (n, 1))      # target_joint_angles (human.py:122); the presets are the same for both genders
         sim.forward_kinematics()
         limb = np.zeros((n, 3, 3))
@@ -243,6 +299,23 @@ class DressingBatch:
         # separately from the steady-state flag, which the caller reads after its own steps
         self.settle_overflow = int(sim.overflow_count()) if hasattr(sim, 'overflow_count') else 0
         return s
+
+    def person_limits(self, links):
+        """Template limits of the person's joints as the per-call Agent sees them (an unlimited joint is +-1e10, agent.py)."""
+        lo, hi = self.scene['link_lower'][links].astype(np.float64), self.scene['link_upper'][links].astype(np.float64)
+        free = (lo == 0) & (hi == -1)
+        return np.where(free, -1e10, lo), np.where(free, 1e10, hi)
+
+    def start_coop(self, sim, sample=None):
+        """Arm the person's half of the fused co-optimisation step (DressingPR2Human-v1); call after `start_fused`.  The arm is
+        driven with the gains take_step's control() issues every step (Human.motor_gains = 0.01 after dressing.py:121, motor_forces
+        1.0); limits are scaled by the sample's `limit_scale`; the classifier of limits_model keeps the left arm inside the
+        realistic joint limits (sign +1: the left arm's input mapping, human.py:141-145)."""
+        from .limits_model import load_model
+        s = sample or self.last_sample
+        P = coop_params(self.scene, self.humans, 3, LEFT_ARM_JOINTS, 0.01)
+        w = pack_mlp(P, load_model(), L_ARM_LIMIT_JOINTS, 1.0)
+        sim.coop_init(P, limit_scale=s.get('limit_scale'), mlp=w)
 
     def start_fused(self, sim, sample=None):
         s = sample or self.last_sample

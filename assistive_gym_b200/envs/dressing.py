@@ -2,11 +2,17 @@
 
 `step` runs the fused path (`ag_dressing_step_host`): action -> PD targets -> 5 x (8 rigid substeps + one cloth launch, the
 cloth's anchor follows the end effector) -> sleeve-on-arm reward, cloth forces, obs[24] / reward / done.  `_get_obs` (used
-by `reset`) reads the same quantities through the per-call Agent API."""
+by `reset`) reads the same quantities through the per-call Agent API.
+
+With a controllable person (co-optimisation, `DressingPR2Human-v1`) `step` takes {'robot': a7, 'human': a10} and goes through the
+per-call path (`step_reference_api`): `take_step` drives the person's left arm and, after every stepSimulation, keeps it inside its
+(per-env scaled) limits and the realistic joint limits (human.py:134-152), then moves the gown's anchor to the end effector
+(`update_targets`); the observation, the sleeve-on-arm reward and the cloth forces are computed on the host.  `step_fused` runs
+the same co-optimisation step on the device (`ag_coop_step_host`).  `tremor` is not drawn for a controllable person."""
 import numpy as np
 
 from .. import capi
-from ..dressing_batch import L_ELBOW, L_SHOULDER, L_WRIST, DressingBatch
+from ..dressing_batch import L_ELBOW, L_SHOULDER, L_WRIST, RADII, TRIANGLE1, TRIANGLE2, DressingBatch, sleeve_on_arm_reward
 from ..sim import BatchSim
 from .env import AssistiveEnv
 
@@ -16,12 +22,18 @@ class DressingEnv(AssistiveEnv):
         super().__init__(robot=robot, human=human, task='dressing', n_envs=n_envs, device=device, seed=seed,
                          obs_robot_len=(17 + len(robot.controllable_joint_indices) - (len(robot.wheel_joint_indices) if robot.mobile else 0)),
                          obs_human_len=(18 + len(human.controllable_joint_indices)))
-        self._db = DressingBatch()
+        self._db = DressingBatch(controllable_person=human.controllable)
         self._cfg = config or DressingBatch.config()                       # numSubSteps = 8 (dressing.py:184)
         self._toc_attempts = toc_attempts
         self._sim_lib = None
 
     def step(self, action):                                                # dressing.py:12-77
+        if self.human.controllable:               # dict in, dicts out (dressing.py:16-17,73-77)
+            a = np.concatenate([np.asarray(action['robot'], dtype=np.float64).reshape(self.n_envs, -1),
+                                np.asarray(action['human'], dtype=np.float64).reshape(self.n_envs, -1)], axis=1)
+            obs, reward, done, info = self.step_reference_api(a)
+            d = bool(np.all(done)) if self.n_envs > 1 else bool(done)
+            return obs, {'robot': reward, 'human': reward}, {'robot': done, 'human': done, '__all__': d}, {'robot': info, 'human': info}
         a = np.asarray(action, dtype=np.float32).reshape(self.n_envs, -1)
         obs, rew, done, info = self.id.dressing_step_host(a)
         self.iteration += 1
@@ -33,6 +45,46 @@ class DressingEnv(AssistiveEnv):
         if self.n_envs == 1:
             return obs[0], float(rew[0]), bool(done[0] > 0.5), {k_: (v[0] if isinstance(v, np.ndarray) else v) for k_, v in out.items()}
         return obs, rew, done > 0.5, out
+
+    def step_fused(self, action):
+        """`step` of the co-optimisation env (DressingPR2Human-v1) on the fused, graph-replayed device path: takes and returns
+        exactly what `step` does.  `step` itself stays on the per-call path."""
+        return self._coop_step_fused(action)
+
+    # ------------------------------------------------------------------ the same step through the reference-shaped API
+    def step_reference_api(self, action):
+        """dressing.py:12-77 through the per-call API: take_step (with the person's limits and the anchor update after every
+        stepSimulation), then the sleeve-on-arm reward, the cloth forces on the person and the observation, on the host."""
+        a = np.asarray(action, dtype=np.float64).reshape(self.n_envs, -1)
+        self.take_step(a)
+        n = self.n_envs
+        x, _ = self.id.cloth_get_state()
+        limb = [p_.astype(np.float64) for p_ in self._arm_points()]
+        forearm, upperarm, reward_dressing = np.zeros(n, dtype=bool), np.zeros(n, dtype=bool), np.zeros(n)
+        for e in range(n):
+            radii = RADII['male' if self.male[e] else 'female']
+            fin, uin, d_fore, d_upper, d_hand, _d_elbow, _d_shoulder, fore_len, upper_len = sleeve_on_arm_reward(
+                x[e, TRIANGLE1], x[e, TRIANGLE2], limb[0][e], limb[1][e], limb[2][e], *radii)
+            if uin:
+                reward_dressing[e] = fore_len + (d_upper if d_upper < upper_len else 0.0)
+            elif fin and d_fore < fore_len:
+                reward_dressing[e] = d_fore
+            else:
+                reward_dressing[e] = -d_hand
+            forearm[e], upperarm[e] = fin, uin
+        self.forearm_in_sleeve, self.upperarm_in_sleeve = forearm, upperarm
+        obs = self._get_obs()
+        ee_vel = np.linalg.norm(np.atleast_2d(self.robot.get_velocity(self.robot.left_end_effector)), axis=1)
+        pref = self.C_v * (-ee_vel) + self.C_d * (-self.cloth_force_sum)          # human_preferences with the dressing forces
+        reward = self.config('dressing_reward_weight') * reward_dressing + self.config('action_weight') * (-np.linalg.norm(a, axis=1)) + pref
+        self.task_success = np.maximum(self.task_success, reward_dressing)
+        done = np.full(n, self.iteration >= 200)
+        info = {'total_force_on_human': self.total_force_on_human, 'task_success': (self.task_success >= self.config('task_success_threshold')).astype(int),
+                'action_robot_len': self.action_robot_len, 'action_human_len': self.action_human_len, 'obs_robot_len': self.obs_robot_len, 'obs_human_len': self.obs_human_len}
+        if n == 1:
+            obs = {k_: v[0] for k_, v in obs.items()} if isinstance(obs, dict) else obs[0]
+            return obs, float(reward[0]), bool(done[0]), {k_: (v[0] if isinstance(v, np.ndarray) else v) for k_, v in info.items()}
+        return obs, reward, done, info
 
     def _arm_points(self):
         out = []
@@ -54,7 +106,24 @@ class DressingEnv(AssistiveEnv):
         self.cloth_force_sum = np.where(keep, f, 0.0).sum(axis=1)
         self.robot_force_on_human = sum(self.id.contact_force_sum(self.robot.body, h.body) for h in self.humans.values()).astype(np.float64)
         self.total_force_on_human = self.robot_force_on_human + self.cloth_force_sum
-        return np.concatenate([ep_r, eq_r, q] + arm + [self.cloth_force_sum[:, None]], axis=1)
+        robot_obs = np.concatenate([ep_r, eq_r, q] + arm + [self.cloth_force_sum[:, None]], axis=1)
+        if agent == 'robot' or not self.human.controllable:
+            return robot_obs
+        # dressing.py:96-105: the end effector, the person's joint angles (not wrapped) and the arm points in the person's base frame
+        def human_frame(pos, orient=None):
+            outs = []
+            for g in ('male', 'female'):
+                r = self.humans[g].convert_to_realworld(pos, orient if orient is not None else np.array([0, 0, 0, 1.0]))
+                outs.append([np.atleast_2d(x) for x in r])
+            return [np.where(self.male[:, None], m, f) for m, f in zip(*outs)]
+        ci = self.human.controllable_joint_indices
+        qh = np.where(self.male[:, None], np.atleast_2d(self.humans['male'].get_joint_angles(ci)), np.atleast_2d(self.humans['female'].get_joint_angles(ci)))
+        ep_h, eq_h = human_frame(ep, eq)
+        arm_h = [human_frame(p_)[0] for p_ in self._arm_points()]
+        human_obs = np.concatenate([ep_h, eq_h, qh] + arm_h + [self.cloth_force_sum[:, None], self.robot_force_on_human[:, None]], axis=1)
+        if agent == 'human':
+            return human_obs
+        return {'robot': robot_obs, 'human': human_obs}
 
     def reset(self):                                                       # dressing.py:108-198
         super().reset()
@@ -67,7 +136,7 @@ class DressingEnv(AssistiveEnv):
             self.furniture.init(db.wheelchair, sim, self.np_random, indices=-1)
             self.humans = {}
             for g, hb in db.humans.items():
-                h = type(self.human)(self.human.controllable_joint_indices, controllable=False)
+                h = type(self.human)(self.human.controllable_joint_indices, controllable=self.human.controllable)
                 h.init(hb, sim, self.np_random, self.human.controllable_joint_indices)
                 self.humans[g] = h
         rng = np.random.default_rng(self.np_random.randint(0, 2 ** 31 - 1))
@@ -77,10 +146,25 @@ class DressingEnv(AssistiveEnv):
         self.male = s['male'].astype(bool)
         self.human.gender = 'male' if self.male[0] else 'female'
         self.start_ee_pos = db.start_ee_pos
+        if self.human.controllable:               # both gender instances act; the switched-off one moves nothing (env.py:130)
+            for g, h in self.humans.items():
+                h.env_mask = self.male if g == 'male' else ~self.male
+                h.arm_previous_valid_pose = {True: None, False: None}
+                h.motor_gains, h.motor_forces = 0.01, 1.0                         # dressing.py:121; Human.motor_forces
+                h.set_limit_scale(s['limit_scale'])                               # impairment 'limits': scaled joint limits (human.py:85)
+                self.agents.append(h)
         db.start_fused(self.id, s)
+        if self.human.controllable:
+            db.start_coop(self.id, s)
         self.task_success = np.zeros(self.n_envs)
         obs = self._get_obs()
+        if isinstance(obs, dict):
+            return {k_: (v[0] if self.n_envs == 1 else v) for k_, v in obs.items()}
         return obs[0] if self.n_envs == 1 else obs
 
     def update_targets(self):                                              # dressing.py:200-210
+        if self.human.controllable:
+            # the person's joint-limit clamps of this stepSimulation move its links (PyBullet's resetJointState does so at once):
+            # the observation and the next stepSimulation's cloth see the clamped poses, as k_fk after k_coop_limits gives them
+            self.id.forward_kinematics()
         self.id.cloth_anchor_follow(self._db.ee_link)

@@ -311,11 +311,11 @@ class BatchSim:
     def scratch_step_dev(self, action_ptr, obs_ptr, reward_ptr, done_ptr, info_ptr):
         self._ck(self.lib.ag_scratch_step_dev(self.h, action_ptr, obs_ptr, reward_ptr, done_ptr, info_ptr))
 
-    # ---- fused co-optimisation path (the person's half; call after feeding_init / scratch_init / bathing_init)
+    # ---- fused co-optimisation path (the person's half; call after feeding_init / scratch_init / bathing_init / dressing_init)
     def coop_init(self, params, limit_scale=None, mlp=None):
         """limit_scale [n] or None; mlp: the packed classifier weights (fp32, agphys.h order) or None"""
         self._coop_params = params
-        self._coop_dims = {0: (25, 23), 1: (30, 34), 2: (24, 28)}.get(int(params.task), (0, 0))
+        self._coop_dims = {0: (25, 23), 1: (30, 34), 2: (24, 28), 3: (24, 28)}.get(int(params.task), (0, 0))
         ls = None if limit_scale is None else np.ascontiguousarray(np.broadcast_to(np.asarray(limit_scale, dtype=np.float64), (self.n,)))
         w = None if mlp is None else np.ascontiguousarray(mlp, dtype=np.float32)
         self._ck(self.lib.ag_coop_init(self.h, C.byref(params), _p(ls), _p(w)))

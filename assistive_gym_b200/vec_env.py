@@ -8,8 +8,9 @@ all envs have the same length (200 steps, feeding.py:37), so the batch resets to
 `step` the way vector-env wrappers do (the terminal observation is kept in `info['terminal_observation']`).
 With numpy inputs the host-buffer entry points are used instead (pinned staging inside the C ABI).
 
-The co-optimisation ids (FeedingJacoHuman-v1, ScratchItchJacoHuman-v1, BedBathingSawyerHuman-v1) run `ag_coop_step_dev`: actions
-are {'robot': [N, 7], 'human': [N, k]}, observations {'robot': [N, 25 | 30 | 24], 'human': [N, 23 | 34 | 28]}, and rewards, dones and infos
+The co-optimisation ids (FeedingJacoHuman-v1, ScratchItchJacoHuman-v1, BedBathingSawyerHuman-v1, DressingPR2Human-v1) run
+`ag_coop_step_dev`: actions are {'robot': [N, 7], 'human': [N, k]}, observations {'robot': [N, 25 | 30 | 24 | 24],
+'human': [N, 23 | 34 | 28 | 28]}, and rewards, dones and infos
 come in the dict shape of the env's `step` (dones with '__all__')."""
 import numpy as np
 
@@ -34,7 +35,7 @@ class AssistiveVecEnv:
         self.task = self.env.task
         self.observation_space, self.action_space = self.env.observation_space, self.env.action_space
         self.obs_dim, self.act_dim = self.observation_space.shape[0], self.action_space.shape[0]
-        self.coop = self.task in ('feeding', 'scratch_itch', 'bed_bathing') and bool(self.env.human.controllable)
+        self.coop = self.task in ('feeding', 'scratch_itch', 'bed_bathing', 'dressing') and bool(self.env.human.controllable)
         self._step_dev = None
         self._buf = None
 

@@ -341,7 +341,7 @@ int ag_scratch_init(AgSim* sim, const AgScratchParams* p, const int32_t* gender_
 int ag_scratch_step_dev(AgSim* sim, const float* action_dev, float* obs_dev, float* reward_dev, float* done_dev, float* info_dev);
 int ag_scratch_step_host(AgSim* sim, const float* action, float* obs, float* reward, float* done, float* info);
 
-/* --- fused co-optimisation step (FeedingJacoHuman-v1, ScratchItchJacoHuman-v1, BedBathingSawyerHuman-v1; env.py:174-235 with the person as a second
+/* --- fused co-optimisation step (FeedingJacoHuman-v1, ScratchItchJacoHuman-v1, BedBathingSawyerHuman-v1, DressingPR2Human-v1; env.py:174-235 with the person as a second
  * agent): the robot part is the task's own fused step; the person's part applies the human slice of the action to its
  * controllable joints (clip to [-1, 1], x 0.05, 5-fold accumulate inside its limits), and after every stepSimulation
  * clamps every joint of the person to its limits (Human.enforce_joint_limits) and, with the classifier on, keeps the arm
@@ -350,12 +350,14 @@ int ag_scratch_step_host(AgSim* sim, const float* action, float* obs, float* rew
 #define AG_COOP_MAXC 10
 typedef struct AgCoopParams {
   int32_t task;                 /* 0 = FeedingEnv (after ag_feeding_init), 1 = ScratchItchEnv (after ag_scratch_init),
-                                   2 = BedBathingEnv (after ag_bathing_init and ag_bathing_set_target_frames) */
+                                   2 = BedBathingEnv (after ag_bathing_init and ag_bathing_set_target_frames),
+                                   3 = DressingEnv (after ag_dressing_init; the left arm, with the gown stepped as in
+                                   ag_dressing_step: after every stepSimulation the limits, then the anchor follows) */
   int32_t human_body_m, human_body_f;
   int32_t n_joints;             /* every joint of the person: enforce_joint_limits clamps all of them */
   int32_t joint_links_m[AG_COOP_MAXJ], joint_links_f[AG_COOP_MAXJ];   /* global link ids per gender */
   double  joint_lower[AG_COOP_MAXJ], joint_upper[AG_COOP_MAXJ];       /* template limits (the `limits` impairment scales them) */
-  int32_t n_ctrl;               /* controllable joints = width of the human part of the action: 4 for feeding, 10 for scratch and bathing */
+  int32_t n_ctrl;               /* controllable joints = width of the human part of the action: 4 for feeding, 10 for scratch, bathing and dressing */
   int32_t ctrl[AG_COOP_MAXC];   /* indices into the joint list */
   float   motor_gain, motor_force;            /* Human.motor_gains / motor_forces: what take_step's control() sets */
   int32_t mlp_slots[4];         /* joint-list indices of shoulder x, y, z and elbow (classifier inputs) */
@@ -367,8 +369,9 @@ typedef struct AgCoopParams {
  * NULL (classifier off).  Resets the per-env last reachable arm pose to "none yet" and sets the person's controllable motors
  * to motor_gain / motor_force (kd 1) in both genders. */
 int ag_coop_init(AgSim* sim, const AgCoopParams* p, const double* limit_scale, const float* mlp);
-/* action [N][7 + n_ctrl] (robot, then person); obs_robot [N][25 | 30 | 24], obs_human [N][23 | 34 | 28], reward [N], done [N],
- * info [N][4] as the task's own step reports them */
+/* action [N][7 + n_ctrl] (robot, then person); obs_robot [N][25 | 30 | 24 | 24], obs_human [N][23 | 34 | 28 | 28] for tasks 0-3,
+ * reward [N], done [N], info [N][4] as the task's own step reports them.  Task 3 refuses a half-done stepSimulation, as
+ * ag_dressing_step does. */
 int ag_coop_step_dev(AgSim* sim, const float* action_dev, float* obs_robot_dev, float* obs_human_dev, float* reward_dev, float* done_dev, float* info_dev);
 int ag_coop_step_host(AgSim* sim, const float* action, float* obs_robot, float* obs_human, float* reward, float* done, float* info);
 /* diagnostic: the device classifier (the function k_coop_limits runs) on host inputs x [n][4] -> p [n] */

@@ -1,11 +1,13 @@
-"""Throughput of the co-optimisation envs (FeedingJacoHuman-v1, ScratchItchJacoHuman-v1, BedBathingSawyerHuman-v1) on one GPU: the fused device step
+"""Throughput of the co-optimisation envs (FeedingJacoHuman-v1, ScratchItchJacoHuman-v1, BedBathingSawyerHuman-v1, DressingPR2Human-v1) on one GPU: the fused device step
 (`step_fused` / ag_coop_step_dev, graph-replayed) against the per-call `step` (take_step + _get_obs through the C ABI, with the
 host round trips of enforce_joint_limits / the realistic-arm-limit classifier after every substep), at the same batch size.
 
 Prints one JSON line per id: fused env-steps/s (CUDA events around the timed steps after warm-up), per-call env-steps/s (a host
 clock around fewer steps, each of which ends in device-to-host reads), k_coop_limits ms per launch (ag_profile_get, in a
 separate profiled run of the fused step; for BedBathing also k_bath_track, which re-places the wiping targets on the moving arm)
-and the card's name and power limit, read in the same run.
+and the card's name and power limit, read in the same run.  Without --n, each id runs at its bench size: 4096 envs, and 2048 for
+DressingPR2Human-v1 (the Dressing bench size); its per-call leg runs at 256 envs (`percall_note`), because the per-call Dressing step
+evaluates the sleeve-on-arm reward env by env on the host.
 
     python tools/gpu_coop_bench.py --n 4096 --steps 50 --warmup 5 --percall-steps 3 [--ids BedBathingSawyerHuman-v1] [--out profiles/h100_coop_bench.jsonl]
 """
@@ -20,6 +22,10 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 import numpy as np  # noqa: E402
+
+
+DEFAULT_N = {'DressingPR2Human-v1': 2048}
+PERCALL_N = {'DressingPR2Human-v1': (256, 'the per-call Dressing step evaluates the sleeve-on-arm reward env by env on the host; measured at 256 envs')}
 
 
 def card():
@@ -77,9 +83,9 @@ def bench(env_id, n, steps, warmup, percall_steps, seed=1001):
     env.close()
     # the per-call path from the same kind of start state (a fresh reset), fewer steps; should it fail at this batch size, it is
     # measured at 1024 envs and the line says so (`percall_n_envs`, `percall_note`)
-    percall_n, note = n, None
+    percall_n, note = PERCALL_N.get(env_id, (n, None))
     try:
-        percall_s = percall(env_id, n, k, percall_steps, seed)
+        percall_s = percall(env_id, percall_n, k, percall_steps, seed)
     except RuntimeError as ex:
         percall_n, note = 1024, 'per-call step fails at %d envs (%s); measured at 1024' % (n, ex)
         percall_s = percall(env_id, percall_n, k, percall_steps, seed)
@@ -112,7 +118,7 @@ def percall(env_id, n, k, steps, seed):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument('--n', type=int, default=4096)
+    ap.add_argument('--n', type=int, default=None, help='envs per id (default: 4096; 2048 for DressingPR2Human-v1)')
     ap.add_argument('--steps', type=int, default=50)
     ap.add_argument('--warmup', type=int, default=5)
     ap.add_argument('--percall-steps', type=int, default=3)
@@ -124,7 +130,8 @@ def main():
         raise SystemExit('no CUDA device: this measurement runs on the GPU only')
     c = card()
     for env_id in args.ids.split(','):
-        r = dict(bench(env_id, args.n, args.steps, args.warmup, args.percall_steps), **c)
+        n = args.n or DEFAULT_N.get(env_id, 4096)
+        r = dict(bench(env_id, n, args.steps, args.warmup, args.percall_steps), **c)
         line = json.dumps(r)
         print(line, flush=True)
         if args.out:
