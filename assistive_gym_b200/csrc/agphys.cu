@@ -160,6 +160,25 @@ static void k_coop_classify(SimDev, KP p) {
 #endif
 
 // ------------------------------------------------------------------ host object
+// The fused tasks, numbered as AgCoopParams.task.  AgSim::io holds one record per task and, at IO_COOP, the
+// co-optimisation step's.
+enum Task { TASK_FEEDING = 0, TASK_SCRATCH = 1, TASK_BATHING = 2, TASK_DRESSING = 3 };
+static const int IO_COOP = 4;
+static const int ROBOT_OBS_W[4] = {25, 30, 24, 24}, HUMAN_OBS_W[4] = {23, 34, 28, 28};   // floats per env, by task
+static const char* const TASK_INIT[4] = {"ag_feeding_init", "ag_scratch_init", "ag_bathing_init", "ag_dressing_init"};
+
+// The outputs of one fused env step; obs_h (the person's observation) only for the co-optimisation step.
+struct StepOut { float *obs, *obs_h, *reward, *done, *info; };
+// One fused-step entry point: its own device buffers (the host-buffer step runs on them, and a captured step reads its
+// action from `action`), pinned staging, and the CUDA graph of its step, keyed by the device pointers it was captured with.
+struct StepGraph { void* exec; const void* key[6]; uint64_t launches; bool valid; };
+struct StepIO {
+  int act_w, obs_w, obs_h_w;           // floats per env of the action, the robot's and the person's observation (0: none)
+  float *action, *obs, *obs_h, *reward, *done, *info;
+  float *host_in, *host_out;           // [N][act_w]; obs, obs_h, reward, done, info [N][4] back to back
+  StepGraph graph;
+};
+
 struct AgSim {
   SimDev S;
   AgConfig cfg;
@@ -178,23 +197,16 @@ struct AgSim {
   FeedDev F; FeedDev* F_dev; bool feeding;
   BathDev B; BathDev* B_dev; bool bathing;
   bool bath_frames;                    // ag_bathing_set_target_frames since the last ag_bathing_init
-  float *h_bpin_in, *h_bpin_out, *d_baction, *d_bobs, *d_breward, *d_bdone, *d_binfo;
-  float *d_action, *d_obs, *d_reward, *d_done, *d_info;
-  float *h_pin_in, *h_pin_out;
   // cloth (Dressing): one k_cloth launch per stepSimulation = `C.K` rigid substeps
   ClothDev C; ClothDev* C_dev; bool cloth; int cloth_sub, cloth_npt, cloth_qs;
   DressPost DP; DressPost* DP_dev; bool dressing;
   ScratchDev SD; ScratchDev* SD_dev; bool scratch;
-  float *h_spin_in, *h_spin_out, *d_saction, *d_sobs, *d_sreward, *d_sdone, *d_sinfo;
   size_t render_pix; int render_n; int* d_render_ids; unsigned char* d_render_rgba; float* d_render_depth; void* d_render_dev;
-  float *h_dpin_in, *h_dpin_out, *d_daction, *d_dobs, *d_dreward, *d_ddone, *d_dinfo;
-  // co-optimisation (the person's half; the robot's half is the feeding / scratch state above)
-  CoopDev CO; CoopDev* CO_dev; bool coop; int coop_width;
-  float *d_caction, *d_cobs_r, *d_cobs_h, *d_creward, *d_cdone, *d_cinfo;
-  float* coop_obs_h;                   // the human-obs buffer the captured coop step writes (not part of the graph key)
-  // CUDA-graph replay of the fused env step (one graph per entry point, keyed by its device pointers)
+  // co-optimisation (the person's half; the robot's half is the task's state above)
+  CoopDev CO; CoopDev* CO_dev; bool coop;
+  // the fused-step entry points (Task, then IO_COOP); CUDA-graph replay of their steps
+  StepIO io[5];
   bool use_graph; int graph_failures;
-  struct StepGraph { void* exec; const void* key[5]; uint64_t launches; bool valid; } graphs[5];
   // profiling
   bool profiling;
   std::vector<std::string> knames;
@@ -207,7 +219,16 @@ struct AgSim {
 #define CKP(x) do { cudaError_t err__ = (x); if (err__ != cudaSuccess) { g_err = std::string(#x) + ": " + cudaGetErrorString(err__); return nullptr; } } while (0)
 #endif
 
-extern "C" { static void drop_graph(AgSim* s, int which); }
+static void drop_graph(StepIO& io) {
+#ifndef AG_CPU_EMU
+  if (io.graph.valid) { cudaGraphExecDestroy((cudaGraphExec_t)io.graph.exec); io.graph.valid = false; }
+#else
+  (void)io;
+#endif
+}
+// A task's init changes what its step captures, and the co-optimisation step runs the task's kernels too: drop both graphs.
+static void drop_task_graphs(AgSim* s, int task) { drop_graph(s->io[task]); drop_graph(s->io[IO_COOP]); }
+static void drop_all_graphs(AgSim* s) { for (StepIO& io : s->io) drop_graph(io); }
 static void* dev_alloc(AgSim* s, size_t bytes) {
   void* p = nullptr;
   if (bytes == 0) bytes = 16;
@@ -349,7 +370,7 @@ AgSim* ag_create(const AgSceneDesc* d, const AgConfig* cfg, int n_envs, int devi
   AgSim* s = new AgSim();
   memset(&s->S, 0, sizeof(SimDev));
   memset(&s->F, 0, sizeof(FeedDev));
-  s->cfg = *cfg; s->device = device; s->launches = 0; s->feeding = false; s->bathing = false; s->cloth = false; s->cloth_sub = 0; s->C_dev = nullptr; s->dressing = false; s->DP_dev = nullptr; s->scratch = false; s->SD_dev = nullptr; s->graphs[3].valid = false; s->render_pix = 0; s->render_n = 0; s->d_render_ids = nullptr; s->d_render_rgba = nullptr; s->d_render_depth = nullptr; s->d_render_dev = nullptr; s->graphs[2].valid = false; s->use_graph = true; s->graph_failures = 0; s->graphs[0].valid = s->graphs[1].valid = false; s->graphs[4].valid = false; s->coop = false; s->CO_dev = nullptr; s->coop_obs_h = nullptr; s->B_dev = nullptr; s->stream = nullptr; s->F_dev = nullptr; s->profiling = false;
+  s->cfg = *cfg; s->device = device; s->launches = 0; s->feeding = false; s->bathing = false; s->cloth = false; s->cloth_sub = 0; s->C_dev = nullptr; s->dressing = false; s->DP_dev = nullptr; s->scratch = false; s->SD_dev = nullptr; s->render_pix = 0; s->render_n = 0; s->d_render_ids = nullptr; s->d_render_rgba = nullptr; s->d_render_depth = nullptr; s->d_render_dev = nullptr; s->use_graph = true; s->graph_failures = 0; s->coop = false; s->CO_dev = nullptr; s->B_dev = nullptr; s->stream = nullptr; s->F_dev = nullptr; s->profiling = false;
   s->d_stage = nullptr; s->stage_floats = 0;
 #ifndef AG_CPU_EMU
   { int ndev = 0; if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) { g_err = "no such CUDA device (is a CUDA device present? there is no CPU fallback)"; delete s; return nullptr; } }
@@ -593,18 +614,14 @@ void ag_destroy(AgSim* s) {
 #ifndef AG_CPU_EMU
   if (s->stream) cudaStreamSynchronize(s->stream);
   for (void* p : s->allocs) cudaFree(p);
-  if (s->feeding) { cudaFreeHost(s->h_pin_in); cudaFreeHost(s->h_pin_out); }
-  if (s->bathing) { cudaFreeHost(s->h_bpin_in); cudaFreeHost(s->h_bpin_out); }
-  if (s->dressing) { cudaFreeHost(s->h_dpin_in); cudaFreeHost(s->h_dpin_out); }
-  if (s->scratch) { cudaFreeHost(s->h_spin_in); cudaFreeHost(s->h_spin_out); }
-  for (int g = 0; g < 5; g++) if (s->graphs[g].valid) cudaGraphExecDestroy((cudaGraphExec_t)s->graphs[g].exec);
+  for (StepIO& io : s->io) {
+    cudaFreeHost(io.host_in); cudaFreeHost(io.host_out);
+    if (io.graph.valid) cudaGraphExecDestroy((cudaGraphExec_t)io.graph.exec);
+  }
   if (s->stream) cudaStreamDestroy(s->stream);
 #else
   for (void* p : s->allocs) free(p);
-  if (s->feeding) { free(s->h_pin_in); free(s->h_pin_out); }
-  if (s->bathing) { free(s->h_bpin_in); free(s->h_bpin_out); }
-  if (s->dressing) { free(s->h_dpin_in); free(s->h_dpin_out); }
-  if (s->scratch) { free(s->h_spin_in); free(s->h_spin_out); }
+  for (StepIO& io : s->io) { free(io.host_in); free(io.host_out); }
 #endif
   delete s;
 }
@@ -775,7 +792,7 @@ int ag_set_motor_force_scale(AgSim* s, int n, const int32_t* links, const float*
     if (!s->S.motor_fscale) return fail("device allocation failed");
     std::vector<float> ones(cnt, 1.0f);
     if (h2d(s, s->S.motor_fscale, ones.data(), cnt * sizeof(float))) return -1;
-    for (int g = 0; g < 5; g++) drop_graph(s, g);        // captured kernels hold the SimDev of before (null pointer)
+    drop_all_graphs(s);                                   // captured kernels hold the SimDev of before (null pointer)
   }
   return scatter_host(s, s->S.motor_fscale, 1, n, links, scale, nullptr);
 }
@@ -1041,34 +1058,151 @@ int ag_overflow_count(AgSim* s) {
   return n;
 }
 
-// ------------------------------------------------------------------ CUDA-graph replay of a fused env step
-// One env step is ~90 small launches (14 kernels + 3 memsets per substep); captured once per set of device
-// pointers and replayed with a single cudaGraphLaunch.  Falls back to direct launches while profiling
-// (per-kernel events), when AG_GRAPH=0, or if capture fails.
-typedef int (*StepEnqueue)(AgSim*, const float*, float*, float*, float*, float*);
-static void drop_graph(AgSim* s, int which) {
-#ifndef AG_CPU_EMU
-  if (s->graphs[which].valid) { cudaGraphExecDestroy((cudaGraphExec_t)s->graphs[which].exec); s->graphs[which].valid = false; }
-#else
-  (void)s; (void)which;
-#endif
+// ------------------------------------------------------------------ the fused env step of every task
+static bool task_ready(const AgSim* s, Task task) {
+  switch (task) {
+    case TASK_FEEDING: return s->feeding;
+    case TASK_SCRATCH: return s->scratch;
+    case TASK_BATHING: return s->bathing;
+    case TASK_DRESSING: return s->dressing;
+  }
+  return false;
 }
-static int run_step(AgSim* s, int which, StepEnqueue enq, const float* action, float* obs, float* reward, float* done, float* info) {
+static void* task_dev(const AgSim* s, Task task) {
+  switch (task) {
+    case TASK_FEEDING: return s->F_dev;
+    case TASK_SCRATCH: return s->SD_dev;
+    case TASK_BATHING: return s->B_dev;
+    case TASK_DRESSING: return s->DP_dev;
+  }
+  return nullptr;
+}
+static int task_frame_skip(const AgSim* s, Task task) {
+  switch (task) {
+    case TASK_FEEDING: return s->F.P.frame_skip;
+    case TASK_SCRATCH: return s->SD.P.frame_skip;
+    case TASK_BATHING: return s->B.P.frame_skip;
+    case TASK_DRESSING: return s->DP.D.P.frame_skip;
+  }
+  return 0;
+}
+static int* task_male(const AgSim* s, Task task) {
+  switch (task) {
+    case TASK_FEEDING: return s->F.male;
+    case TASK_SCRATCH: return s->SD.male;
+    case TASK_BATHING: return s->B.male;
+    case TASK_DRESSING: return s->DP.D.male;
+  }
+  return nullptr;
+}
+
+// An entry point's buffers, allocated at its first init: device buffers, then pinned staging for the host-buffer step.
+static int io_alloc(AgSim* s, StepIO& io, int act_w, int obs_w, int obs_h_w) {
+  const size_t N = s->S.N;
+  io.act_w = act_w; io.obs_w = obs_w; io.obs_h_w = obs_h_w;
+  io.action = dalloc<float>(s, N * act_w); io.obs = dalloc<float>(s, N * obs_w);
+  io.obs_h = obs_h_w ? dalloc<float>(s, N * obs_h_w) : nullptr;
+  io.reward = dalloc<float>(s, N); io.done = dalloc<float>(s, N); io.info = dalloc<float>(s, N * 4);
+  if (!io.action || !io.obs || (obs_h_w && !io.obs_h) || !io.reward || !io.done || !io.info) return fail("device allocation failed");
+  const size_t in = sizeof(float) * N * act_w, out = sizeof(float) * N * (obs_w + obs_h_w + 6);
+#ifndef AG_CPU_EMU
+  CK(cudaMallocHost((void**)&io.host_in, in));
+  CK(cudaMallocHost((void**)&io.host_out, out));
+#else
+  io.host_in = (float*)malloc(in); io.host_out = (float*)malloc(out);
+#endif
+  return 0;
+}
+
+static size_t coop_smem_bytes(bool mlp) { return mlp ? (size_t)(AG_MLP_FLOATS + 2 * AG_MLP_H * AG_COOP_T) * sizeof(float) : 0; }
+static void coop_limits_launch(AgSim* s) {
+  KP p = kp0(); p.n = s->S.N; p.p1 = s->CO_dev;
+#ifndef AG_CPU_EMU
+  int ps = s->profiling ? prof_slot(s, "k_coop_limits") : -1;
+  if (ps >= 0) prof_mark(s, ps, true);
+  k_coop_limits<<<(p.n + AG_COOP_T - 1) / AG_COOP_T, AG_COOP_T, coop_smem_bytes(s->CO.mlp_on), s->stream>>>(s->S, p);
+  if (ps >= 0) prof_mark(s, ps, false);
+#else
+  k_coop_limits(s->S, p);
+#endif
+  s->launches++;
+}
+
+// One env step of `task`: its pre kernel, frame_skip stepSimulations, its after-step kernels and its post kernel.  With `coop`
+// the person is a second agent (ag_coop.cuh): the person's action after the task's pre kernel, the person's limits after every
+// stepSimulation, the person's observation last; the pre / post kernels then read an action row of 7 + n_ctrl floats.
+static int fused_enqueue(AgSim* s, Task task, bool coop, const float* action, const StepOut& o) {
+  const int N = s->S.N, k = coop ? s->CO.P.n_ctrl : 0;
+  void* dev = task_dev(s, task);
+  KP p = kp0(); p.p0 = action; p.p1 = dev; p.i0 = k;
+  switch (task) {
+    case TASK_FEEDING: LAUNCH(s, k_feed_pre, N, p); break;
+    case TASK_SCRATCH: LAUNCH(s, k_scratch_pre, N, p); break;
+    case TASK_BATHING: LAUNCH(s, k_bath_pre, N, p); break;
+    case TASK_DRESSING: LAUNCH(s, k_dress_pre, N, p); break;
+  }
+  if (coop) {
+    KP c = kp0(); c.p0 = action; c.p1 = s->CO_dev;
+    LAUNCH(s, k_coop_pre, N, c);
+  }
+  const int sub = s->cfg.num_substeps > 0 ? s->cfg.num_substeps : 1;
+  const int frames = coop ? s->CO.frame_skip : task_frame_skip(s, task);
+  KP z = kp0();
+  for (int f = 0; f < frames; f++) {                   // stepSimulation, then the person's limits (env.py:223-231)
+    for (int i = 0; i < sub; i++) substep(s);          // with a cloth, the last one launches k_cloth
+    if (coop) coop_limits_launch(s);
+    if (task == TASK_DRESSING) {     // then update_targets (dressing.py:210): the gown's anchor goes to the end effector
+      LAUNCH(s, k_fk, (size_t)s->S.nb * N, z);         // k_coop_limits' restored poses are what the next cloth snapshot sees
+      KP a = kp0(); a.p0 = s->C_dev; a.i0 = s->DP.D.P.ee_link;
+      LAUNCH(s, k_cloth_follow, N, a);
+    }
+  }
+  if (task != TASK_DRESSING) LAUNCH(s, k_fk, (size_t)s->S.nb * N, z);
+  if (task == TASK_FEEDING || task == TASK_BATHING) {
+    KP a = kp0(); a.p0 = s->S.movcol; a.i0 = s->S.nmovcol;
+    LAUNCH(s, k_aabb, (size_t)s->S.nmovcol * N, a);
+    KP l = kp0(); l.p0 = s->S.movlink; l.i0 = s->S.nmovlink;
+    LAUNCH(s, k_linkaabb, (size_t)s->S.nmovlink * N, l);
+  }
+  KP t = kp0(); t.p1 = dev;
+  KP q = kp0(); q.p0 = action; q.p1 = dev; q.p2 = o.obs; q.p3 = o.reward; q.p4 = o.done; q.p5 = o.info; q.i0 = k;
+  switch (task) {
+    case TASK_FEEDING:
+      LAUNCH(s, k_feed_food, (size_t)N * s->F.P.n_foods, t);
+      LAUNCH(s, k_feed_post, N, q);
+      break;
+    case TASK_SCRATCH: LAUNCH(s, k_scratch_post, N, q); break;
+    case TASK_BATHING:   // with a moving person the targets follow the arm (update_targets), k_coop_limits' restorations included
+      if (coop) LAUNCH(s, k_bath_track, (size_t)N * s->B.P.n_targets_max, t);
+      LAUNCH(s, k_bath_dist, (size_t)N * s->B.n_slots, t);
+      LAUNCH(s, k_bath_post, N, q);
+      break;
+    case TASK_DRESSING: LAUNCH(s, k_dress_post, N, q); break;
+  }
+  if (coop) {
+    KP h = kp0(); h.p1 = s->CO_dev; h.p2 = dev; h.p3 = o.obs_h; h.p4 = o.info;
+    LAUNCH(s, k_coop_obs, N, h);
+  }
+  return 0;
+}
+
+// CUDA-graph replay: one env step is ~90 small launches (14 kernels + 3 memsets per substep); captured once per set of device
+// pointers and replayed with a single cudaGraphLaunch.  Falls back to direct launches while profiling (per-kernel events),
+// when AG_GRAPH=0, or if capture fails.
+static int run_step(AgSim* s, StepIO& io, Task task, bool coop, const float* action, const StepOut& o) {
 #ifndef AG_CPU_EMU
   if (s->use_graph && !s->profiling) {
-    // The graph is captured against the sim's OWN action buffer: a learner hands in a freshly allocated action tensor
-    // every step, and a graph keyed on that address would be re-captured (~90 launches + instantiate) each time.
-    float* own = which == 0 ? s->d_action : (which == 1 ? s->d_baction : (which == 2 ? s->d_daction : (which == 3 ? s->d_saction : s->d_caction)));
-    const size_t width = which == 4 ? (size_t)s->coop_width : 7;
-    if (action != own) { CK(cudaMemcpyAsync(own, action, sizeof(float) * width * s->S.N, cudaMemcpyDeviceToDevice, s->stream)); action = own; }
-    AgSim::StepGraph& G = s->graphs[which];
-    const void* key[5] = {action, obs, reward, done, info};
+    // The graph is captured against the entry point's OWN action buffer: a learner hands in a freshly allocated action
+    // tensor every step, and a graph keyed on that address would be re-captured (~90 launches + instantiate) each time.
+    if (action != io.action) { CK(cudaMemcpyAsync(io.action, action, sizeof(float) * io.act_w * s->S.N, cudaMemcpyDeviceToDevice, s->stream)); action = io.action; }
+    StepGraph& G = io.graph;
+    const void* key[6] = {action, o.obs, o.obs_h, o.reward, o.done, o.info};
     if (G.valid && memcmp(G.key, key, sizeof(key)) != 0) { cudaGraphExecDestroy((cudaGraphExec_t)G.exec); G.valid = false; }
     if (!G.valid) {
       uint64_t l0 = s->launches;
       cudaGraph_t graph = nullptr; cudaGraphExec_t exec = nullptr;
       if (cudaStreamBeginCapture(s->stream, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
-        int rc = enq(s, action, obs, reward, done, info);
+        int rc = fused_enqueue(s, task, coop, action, o);
         cudaError_t ce = cudaStreamEndCapture(s->stream, &graph);
         if (rc == 0 && ce == cudaSuccess && graph && cudaGraphInstantiate(&exec, graph, 0) == cudaSuccess) {
           G.exec = exec; memcpy(G.key, key, sizeof(key)); G.launches = s->launches - l0; G.valid = true; s->graph_failures = 0;
@@ -1085,9 +1219,69 @@ static int run_step(AgSim* s, int which, StepEnqueue enq, const float* action, f
     }
   }
 #else
-  (void)which;
+  (void)io;
 #endif
-  return enq(s, action, obs, reward, done, info);
+  return fused_enqueue(s, task, coop, action, o);
+}
+
+static int step_check(const AgSim* s, Task task, bool coop) {
+  if (coop && !s->coop) return fail("ag_coop_init not called");
+  if (!task_ready(s, task)) return fail(std::string(TASK_INIT[task]) + " not called");
+  if (coop && task == TASK_BATHING && !s->bath_frames) return fail("ag_coop_step: call ag_bathing_set_target_frames after ag_bathing_init");
+  if (task == TASK_DRESSING && s->cloth_sub != 0) return fail("fused dressing step: a stepSimulation is half done (ag_step with a partial substep count?)");
+  return 0;
+}
+static StepIO& step_io(AgSim* s, Task task, bool coop) { return s->io[coop ? IO_COOP : task]; }
+
+// the device-pointer step: enqueued on the sim's stream
+static int step_dev(AgSim* s, Task task, bool coop, const float* action, const StepOut& o) {
+  if (step_check(s, task, coop)) return -1;
+  int rc = run_step(s, step_io(s, task, coop), task, coop, action, o);
+#ifndef AG_CPU_EMU
+  CK(cudaGetLastError());
+#endif
+  return rc;
+}
+static int copy_async(AgSim* s, void* dst, const void* src, size_t bytes) {
+#ifndef AG_CPU_EMU
+  CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, s->stream));
+#else
+  (void)s; memcpy(dst, src, bytes);
+#endif
+  return 0;
+}
+// The host-buffer step in two halves: `host_begin` stages the actions (pinned) and enqueues H2D, the fused step and the D2H
+// read-back on the sim's stream and returns; `host_end` waits for that stream and hands the results out.  Several sims
+// (sub-batches of one batch, each on its own stream) overlap this way.
+static int host_begin(AgSim* s, Task task, bool coop, const float* action) {
+  if (step_check(s, task, coop)) return -1;
+  StepIO& io = step_io(s, task, coop);
+  const size_t N = s->S.N;
+  memcpy(io.host_in, action, sizeof(float) * N * io.act_w);
+  if (copy_async(s, io.action, io.host_in, sizeof(float) * N * io.act_w)) return -1;
+  if (run_step(s, io, task, coop, io.action, StepOut{io.obs, io.obs_h, io.reward, io.done, io.info})) return -1;
+  const float* src[5] = {io.obs, io.obs_h, io.reward, io.done, io.info};
+  const int w[5] = {io.obs_w, io.obs_h_w, 1, 1, 4};
+  float* h = io.host_out;
+  for (int i = 0; i < 5; h += N * w[i], i++) if (w[i] && copy_async(s, h, src[i], sizeof(float) * N * w[i])) return -1;
+  return 0;
+}
+static int host_end(AgSim* s, Task task, bool coop, const StepOut& o) {
+  if (step_check(s, task, coop)) return -1;
+  const StepIO& io = step_io(s, task, coop);
+#ifndef AG_CPU_EMU
+  CK(cudaStreamSynchronize(s->stream));
+  CK(cudaGetLastError());
+#endif
+  const size_t N = s->S.N;
+  float* dst[5] = {o.obs, o.obs_h, o.reward, o.done, o.info};      // info may be NULL
+  const int w[5] = {io.obs_w, io.obs_h_w, 1, 1, 4};
+  const float* h = io.host_out;
+  for (int i = 0; i < 5; h += N * w[i], i++) if (w[i] && dst[i]) memcpy(dst[i], h, sizeof(float) * N * w[i]);
+  return 0;
+}
+static int host_step(AgSim* s, Task task, bool coop, const float* action, const StepOut& o) {
+  return host_begin(s, task, coop, action) ? -1 : host_end(s, task, coop, o);
 }
 
 // ------------------------------------------------------------------ cloth (K8, ag_cloth.cuh)
@@ -1194,7 +1388,7 @@ int ag_cloth_init(AgSim* s, const AgClothDesc* d) {
   if (s->cloth_npt == 4) { CK(cudaFuncSetAttribute(k_cloth<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); CK(cudaFuncSetAttribute(k_cloth<4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); }
   else { CK(cudaFuncSetAttribute(k_cloth<8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); CK(cudaFuncSetAttribute(k_cloth<8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); }
 #endif
-  drop_graph(s, 0); drop_graph(s, 1); drop_graph(s, 2); drop_graph(s, 4);
+  drop_all_graphs(s);                  // the captured substeps launch no k_cloth yet
   s->cloth = true; s->cloth_sub = 0;
   return 0;
 }
@@ -1250,8 +1444,7 @@ int ag_cloth_set_gravity(AgSim* s, const double g[3]) {
   DevGuard guard__(s->device);
   if (!s->cloth) return fail("ag_cloth_init not called");
   s->C.gx = (float)g[0]; s->C.gy = (float)g[1]; s->C.gz = (float)g[2];
-  // k_cloth takes ClothDev by value: a captured step (the fused steps and the co-optimisation step) holds the old gravity
-  drop_graph(s, 0); drop_graph(s, 1); drop_graph(s, 2); drop_graph(s, 4);
+  drop_all_graphs(s);                  // k_cloth takes ClothDev by value: a captured step holds the old gravity
   return cloth_refresh(s);
 }
 int ag_cloth_get_contacts(AgSim* s, int max_pts, int32_t* count, int32_t* node, float* pos, float* force, int32_t* link) {
@@ -1301,21 +1494,14 @@ int ag_dressing_init(AgSim* s, const AgDressingParams* p, const int32_t* gender_
   if (p->ee_link < 0 || p->ee_link >= s->nl) return fail("ag_dressing_init: bad end effector link");
   DressDev& D = s->DP.D;
   D.P = *p;
-  drop_graph(s, 2); drop_graph(s, 4);     // the Dressing co-optimisation step captures ee_link and frame_skip as well
+  drop_task_graphs(s, TASK_DRESSING);
   if (!s->dressing) {
     D.male = dalloc<int>(s, N); D.iteration = dalloc<int>(s, N); D.task_success = dalloc<float>(s, N); D.action = dalloc<float>(s, (size_t)N * 7);
     D.tremor_on = dalloc<int>(s, N); D.tremor_rest = dalloc<float>(s, (size_t)N * 10); D.tremor_amp = dalloc<float>(s, (size_t)N * 10);
     D.person_force = dalloc<float>(s, (size_t)N * 2);
-    s->d_daction = dalloc<float>(s, (size_t)N * 7); s->d_dobs = dalloc<float>(s, (size_t)N * 24);
-    s->d_dreward = dalloc<float>(s, N); s->d_ddone = dalloc<float>(s, N); s->d_dinfo = dalloc<float>(s, (size_t)N * 4);
     s->DP_dev = dalloc<DressPost>(s, 1);
-    if (!s->d_dinfo || !s->DP_dev || !D.person_force) return fail("device allocation failed");
-#ifndef AG_CPU_EMU
-    CK(cudaMallocHost((void**)&s->h_dpin_in, sizeof(float) * N * 7));
-    CK(cudaMallocHost((void**)&s->h_dpin_out, sizeof(float) * N * 30));
-#else
-    s->h_dpin_in = (float*)malloc(sizeof(float) * N * 7); s->h_dpin_out = (float*)malloc(sizeof(float) * N * 30);
-#endif
+    if (!s->DP_dev || !D.person_force) return fail("device allocation failed");
+    if (io_alloc(s, s->io[TASK_DRESSING], 7, ROBOT_OBS_W[TASK_DRESSING], 0)) return -1;
   }
   else if (dev_zero(s, D.tremor_on, sizeof(int) * N)) return -1;
   for (int j = 0; j < 10; j++) if (p->human_arm_m[j] < 0 || p->human_arm_m[j] >= s->nl || p->human_arm_f[j] < 0 || p->human_arm_f[j] >= s->nl) return fail("ag_dressing_init: bad human arm link");
@@ -1337,57 +1523,13 @@ int ag_dressing_set_tremor(AgSim* s, const int32_t* on, const float* rest, const
   if (h2d(s, s->DP.D.tremor_on, o.data(), sizeof(int) * N) || h2d(s, s->DP.D.tremor_rest, r.data(), sizeof(float) * 10 * N)) return -1;
   return h2d(s, s->DP.D.tremor_amp, a.data(), sizeof(float) * 10 * N);
 }
-static int dressing_step_enqueue(AgSim* s, const float* action_dev, float* obs, float* reward, float* done, float* info) {
-  const int N = s->S.N;
-  KP p = kp0(); p.p0 = action_dev; p.p1 = s->DP_dev;
-  LAUNCH(s, k_dress_pre, N, p);
-  const int sub = s->cfg.num_substeps > 0 ? s->cfg.num_substeps : 1;
-  KP z = kp0();
-  for (int f = 0; f < s->DP.D.P.frame_skip; f++) {
-    for (int i = 0; i < sub; i++) substep(s);                        // the last one launches k_cloth
-    LAUNCH(s, k_fk, (size_t)s->S.nb * N, z);
-    KP c = kp0(); c.p0 = s->C_dev; c.i0 = s->DP.D.P.ee_link;         // update_targets (dressing.py:210)
-    LAUNCH(s, k_cloth_follow, N, c);
-  }
-  KP q = kp0(); q.p0 = action_dev; q.p1 = s->DP_dev; q.p2 = obs; q.p3 = reward; q.p4 = done; q.p5 = info;
-  LAUNCH(s, k_dress_post, N, q);
-  return 0;
-}
 int ag_dressing_step_dev(AgSim* s, const float* action_dev, float* obs_dev, float* reward_dev, float* done_dev, float* info_dev) {
   DevGuard guard__(s->device);
-  if (!s->dressing) return fail("ag_dressing_init not called");
-  if (s->cloth_sub != 0) return fail("ag_dressing_step: a stepSimulation is half done (ag_step with a partial substep count?)");
-  int rc = run_step(s, 2, dressing_step_enqueue, action_dev, obs_dev, reward_dev, done_dev, info_dev);
-#ifndef AG_CPU_EMU
-  CK(cudaGetLastError());
-#endif
-  return rc;
+  return step_dev(s, TASK_DRESSING, false, action_dev, StepOut{obs_dev, nullptr, reward_dev, done_dev, info_dev});
 }
 int ag_dressing_step_host(AgSim* s, const float* action, float* obs, float* reward, float* done, float* info) {
   DevGuard guard__(s->device);
-  if (!s->dressing) return fail("ag_dressing_init not called");
-  const int N = s->S.N;
-  memcpy(s->h_dpin_in, action, sizeof(float) * N * 7);
-#ifndef AG_CPU_EMU
-  CK(cudaMemcpyAsync(s->d_daction, s->h_dpin_in, sizeof(float) * N * 7, cudaMemcpyHostToDevice, s->stream));
-#else
-  memcpy(s->d_daction, s->h_dpin_in, sizeof(float) * N * 7);
-#endif
-  if (ag_dressing_step_dev(s, s->d_daction, s->d_dobs, s->d_dreward, s->d_ddone, s->d_dinfo)) return -1;
-  float* o = s->h_dpin_out;
-#ifndef AG_CPU_EMU
-  CK(cudaMemcpyAsync(o, s->d_dobs, sizeof(float) * N * 24, cudaMemcpyDeviceToHost, s->stream));
-  CK(cudaMemcpyAsync(o + (size_t)N * 24, s->d_dreward, sizeof(float) * N, cudaMemcpyDeviceToHost, s->stream));
-  CK(cudaMemcpyAsync(o + (size_t)N * 25, s->d_ddone, sizeof(float) * N, cudaMemcpyDeviceToHost, s->stream));
-  CK(cudaMemcpyAsync(o + (size_t)N * 26, s->d_dinfo, sizeof(float) * N * 4, cudaMemcpyDeviceToHost, s->stream));
-  CK(cudaStreamSynchronize(s->stream));
-#else
-  memcpy(o, s->d_dobs, sizeof(float) * N * 24); memcpy(o + (size_t)N * 24, s->d_dreward, sizeof(float) * N);
-  memcpy(o + (size_t)N * 25, s->d_ddone, sizeof(float) * N); memcpy(o + (size_t)N * 26, s->d_dinfo, sizeof(float) * N * 4);
-#endif
-  memcpy(obs, o, sizeof(float) * N * 24); memcpy(reward, o + (size_t)N * 24, sizeof(float) * N);
-  memcpy(done, o + (size_t)N * 25, sizeof(float) * N); memcpy(info, o + (size_t)N * 26, sizeof(float) * N * 4);
-  return 0;
+  return host_step(s, TASK_DRESSING, false, action, StepOut{obs, nullptr, reward, done, info});
 }
 
 // ------------------------------------------------------------------ camera images (K9, ag_render.cuh)
@@ -1435,20 +1577,13 @@ int ag_scratch_init(AgSim* s, const AgScratchParams* p, const int32_t* gender_is
   for (int e = 0; e < N; e++) if (limb_link[e] < 0 || limb_link[e] >= s->nl) return fail("ag_scratch_init: bad limb link");
   ScratchDev& D = s->SD;
   D.P = *p;
-  drop_graph(s, 3); drop_graph(s, 4);
+  drop_task_graphs(s, TASK_SCRATCH);
   if (!s->scratch) {
     D.male = dalloc<int>(s, N); D.iteration = dalloc<int>(s, N); D.task_success = dalloc<int>(s, N); D.limb_link = dalloc<int>(s, N);
     D.target_local = dalloc<float>(s, (size_t)3 * N); D.prev_contact = dalloc<float>(s, (size_t)3 * N); D.action = dalloc<float>(s, (size_t)7 * N);
-    s->d_saction = dalloc<float>(s, (size_t)N * 7); s->d_sobs = dalloc<float>(s, (size_t)N * 30);
-    s->d_sreward = dalloc<float>(s, N); s->d_sdone = dalloc<float>(s, N); s->d_sinfo = dalloc<float>(s, (size_t)N * 4);
     s->SD_dev = dalloc<ScratchDev>(s, 1);
-    if (!s->d_sinfo || !s->SD_dev) return fail("device allocation failed");
-#ifndef AG_CPU_EMU
-    CK(cudaMallocHost((void**)&s->h_spin_in, sizeof(float) * N * 7));
-    CK(cudaMallocHost((void**)&s->h_spin_out, sizeof(float) * N * 36));
-#else
-    s->h_spin_in = (float*)malloc(sizeof(float) * N * 7); s->h_spin_out = (float*)malloc(sizeof(float) * N * 36);
-#endif
+    if (!s->SD_dev) return fail("device allocation failed");
+    if (io_alloc(s, s->io[TASK_SCRATCH], 7, ROBOT_OBS_W[TASK_SCRATCH], 0)) return -1;
   }
   std::vector<float> tl((size_t)3 * N);
   for (int e = 0; e < N; e++) for (int c = 0; c < 3; c++) tl[(size_t)c * N + e] = target_local[(size_t)e * 3 + c];
@@ -1458,51 +1593,13 @@ int ag_scratch_init(AgSim* s, const AgScratchParams* p, const int32_t* gender_is
   s->scratch = true;
   return 0;
 }
-static int scratch_step_enqueue(AgSim* s, const float* action_dev, float* obs, float* reward, float* done, float* info) {
-  const int N = s->S.N;
-  KP p = kp0(); p.p0 = action_dev; p.p1 = s->SD_dev;
-  LAUNCH(s, k_scratch_pre, N, p);
-  for (int i = 0; i < s->SD.P.frame_skip * (s->cfg.num_substeps > 0 ? s->cfg.num_substeps : 1); i++) substep(s);
-  KP z = kp0();
-  LAUNCH(s, k_fk, (size_t)s->S.nb * N, z);
-  KP q = kp0(); q.p0 = action_dev; q.p1 = s->SD_dev; q.p2 = obs; q.p3 = reward; q.p4 = done; q.p5 = info;
-  LAUNCH(s, k_scratch_post, N, q);
-  return 0;
-}
 int ag_scratch_step_dev(AgSim* s, const float* action_dev, float* obs_dev, float* reward_dev, float* done_dev, float* info_dev) {
   DevGuard guard__(s->device);
-  if (!s->scratch) return fail("ag_scratch_init not called");
-  int rc = run_step(s, 3, scratch_step_enqueue, action_dev, obs_dev, reward_dev, done_dev, info_dev);
-#ifndef AG_CPU_EMU
-  CK(cudaGetLastError());
-#endif
-  return rc;
+  return step_dev(s, TASK_SCRATCH, false, action_dev, StepOut{obs_dev, nullptr, reward_dev, done_dev, info_dev});
 }
 int ag_scratch_step_host(AgSim* s, const float* action, float* obs, float* reward, float* done, float* info) {
   DevGuard guard__(s->device);
-  if (!s->scratch) return fail("ag_scratch_init not called");
-  const int N = s->S.N;
-  memcpy(s->h_spin_in, action, sizeof(float) * N * 7);
-#ifndef AG_CPU_EMU
-  CK(cudaMemcpyAsync(s->d_saction, s->h_spin_in, sizeof(float) * N * 7, cudaMemcpyHostToDevice, s->stream));
-#else
-  memcpy(s->d_saction, s->h_spin_in, sizeof(float) * N * 7);
-#endif
-  if (ag_scratch_step_dev(s, s->d_saction, s->d_sobs, s->d_sreward, s->d_sdone, s->d_sinfo)) return -1;
-  float* o = s->h_spin_out;
-#ifndef AG_CPU_EMU
-  CK(cudaMemcpyAsync(o, s->d_sobs, sizeof(float) * N * 30, cudaMemcpyDeviceToHost, s->stream));
-  CK(cudaMemcpyAsync(o + (size_t)N * 30, s->d_sreward, sizeof(float) * N, cudaMemcpyDeviceToHost, s->stream));
-  CK(cudaMemcpyAsync(o + (size_t)N * 31, s->d_sdone, sizeof(float) * N, cudaMemcpyDeviceToHost, s->stream));
-  CK(cudaMemcpyAsync(o + (size_t)N * 32, s->d_sinfo, sizeof(float) * N * 4, cudaMemcpyDeviceToHost, s->stream));
-  CK(cudaStreamSynchronize(s->stream));
-#else
-  memcpy(o, s->d_sobs, sizeof(float) * N * 30); memcpy(o + (size_t)N * 30, s->d_sreward, sizeof(float) * N);
-  memcpy(o + (size_t)N * 31, s->d_sdone, sizeof(float) * N); memcpy(o + (size_t)N * 32, s->d_sinfo, sizeof(float) * N * 4);
-#endif
-  memcpy(obs, o, sizeof(float) * N * 30); memcpy(reward, o + (size_t)N * 30, sizeof(float) * N);
-  memcpy(done, o + (size_t)N * 31, sizeof(float) * N); memcpy(info, o + (size_t)N * 32, sizeof(float) * N * 4);
-  return 0;
+  return host_step(s, TASK_SCRATCH, false, action, StepOut{obs, nullptr, reward, done, info});
 }
 
 // ------------------------------------------------------------------ fused FeedingEnv path
@@ -1512,22 +1609,15 @@ int ag_feeding_init(AgSim* s, const AgFeedingParams* p, const int32_t* gender_is
   FeedDev& F = s->F;
   F.P = *p;
   if (p->n_foods > 16) return fail("too many foods");
-  drop_graph(s, 0); drop_graph(s, 4);    // the captured steps refer to the previous FeedDev
+  drop_task_graphs(s, TASK_FEEDING);     // the captured steps refer to the previous FeedDev
   if (!s->feeding) {          // buffers are allocated once; a later init (episode reset) only refreshes their contents
     F.male = dalloc<int>(s, N); F.food_state = dalloc<int>(s, N); F.iteration = dalloc<int>(s, N); F.task_success = dalloc<int>(s, N);
     F.food_near = dalloc<int>(s, (size_t)N * 16);
     F.action = dalloc<float>(s, (size_t)N * 7); F.rng = dalloc<unsigned long long>(s, N);
     F.tremor_on = dalloc<int>(s, N); F.tremor_rest = dalloc<float>(s, (size_t)N * 4); F.tremor_amp = dalloc<float>(s, (size_t)N * 4);
-    s->d_action = dalloc<float>(s, (size_t)N * 7); s->d_obs = dalloc<float>(s, (size_t)N * 25);
-    s->d_reward = dalloc<float>(s, N); s->d_done = dalloc<float>(s, N); s->d_info = dalloc<float>(s, (size_t)N * 4);
     s->F_dev = dalloc<FeedDev>(s, 1);
-    if (!s->d_info || !s->F_dev) return fail("device allocation failed");
-#ifndef AG_CPU_EMU
-    CK(cudaMallocHost((void**)&s->h_pin_in, sizeof(float) * N * 7));
-    CK(cudaMallocHost((void**)&s->h_pin_out, sizeof(float) * N * 31));
-#else
-    s->h_pin_in = (float*)malloc(sizeof(float) * N * 7); s->h_pin_out = (float*)malloc(sizeof(float) * N * 31);
-#endif
+    if (!s->F_dev) return fail("device allocation failed");
+    if (io_alloc(s, s->io[TASK_FEEDING], 7, ROBOT_OBS_W[TASK_FEEDING], 0)) return -1;
   } else {
     if (dev_zero(s, F.tremor_on, sizeof(int) * N) || dev_zero(s, F.rng, sizeof(unsigned long long) * N)) return -1;
   }
@@ -1567,74 +1657,21 @@ int ag_feeding_reset_episode(AgSim* s, const int32_t* env_mask) {
   return 0;
 }
 
-static int feeding_step_enqueue(AgSim* s, const float* action_dev, float* obs, float* reward, float* done, float* info) {
-  const int N = s->S.N;
-  KP p = kp0(); p.p0 = action_dev; p.p1 = s->F_dev;
-  LAUNCH(s, k_feed_pre, N, p);
-  for (int i = 0; i < s->F.P.frame_skip * (s->cfg.num_substeps > 0 ? s->cfg.num_substeps : 1); i++) substep(s);
-  KP z = kp0();
-  LAUNCH(s, k_fk, (size_t)s->S.nb * N, z);
-  KP a = kp0(); a.p0 = s->S.movcol; a.i0 = s->S.nmovcol;
-  LAUNCH(s, k_aabb, (size_t)s->S.nmovcol * N, a);
-  KP l = kp0(); l.p0 = s->S.movlink; l.i0 = s->S.nmovlink;
-  LAUNCH(s, k_linkaabb, (size_t)s->S.nmovlink * N, l);
-  KP f = kp0(); f.p1 = s->F_dev;
-  LAUNCH(s, k_feed_food, (size_t)N * s->F.P.n_foods, f);
-  KP q = kp0(); q.p0 = action_dev; q.p1 = s->F_dev; q.p2 = obs; q.p3 = reward; q.p4 = done; q.p5 = info;
-  LAUNCH(s, k_feed_post, N, q);
-  return 0;
-}
 int ag_feeding_step_dev(AgSim* s, const float* action_dev, float* obs_dev, float* reward_dev, float* done_dev, float* info_dev) {
   DevGuard guard__(s->device);
-  if (!s->feeding) return fail("ag_feeding_init not called");
-  int rc = run_step(s, 0, feeding_step_enqueue, action_dev, obs_dev, reward_dev, done_dev, info_dev);
-#ifndef AG_CPU_EMU
-  CK(cudaGetLastError());
-#endif
-  return rc;
+  return step_dev(s, TASK_FEEDING, false, action_dev, StepOut{obs_dev, nullptr, reward_dev, done_dev, info_dev});
 }
-// host-buffer step in two halves: `begin` stages the actions (pinned) and enqueues H2D, the fused step and the D2H
-// read-back on the sim's stream and returns; `end` waits for that stream and hands the results out.  Several sims
-// (sub-batches of one batch, each on its own stream) overlap this way; ag_feeding_step_host = begin + end.
+int ag_feeding_step_host(AgSim* s, const float* action, float* obs, float* reward, float* done, float* info) {
+  DevGuard guard__(s->device);
+  return host_step(s, TASK_FEEDING, false, action, StepOut{obs, nullptr, reward, done, info});
+}
 int ag_feeding_step_host_begin(AgSim* s, const float* action) {
   DevGuard guard__(s->device);
-  if (!s->feeding) return fail("ag_feeding_init not called");
-  const int N = s->S.N;
-  memcpy(s->h_pin_in, action, sizeof(float) * N * 7);
-#ifndef AG_CPU_EMU
-  CK(cudaMemcpyAsync(s->d_action, s->h_pin_in, sizeof(float) * N * 7, cudaMemcpyHostToDevice, s->stream));
-#else
-  memcpy(s->d_action, s->h_pin_in, sizeof(float) * N * 7);
-#endif
-  if (run_step(s, 0, feeding_step_enqueue, s->d_action, s->d_obs, s->d_reward, s->d_done, s->d_info)) return -1;
-#ifndef AG_CPU_EMU
-  CK(cudaMemcpyAsync(s->h_pin_out, s->d_obs, sizeof(float) * N * 25, cudaMemcpyDeviceToHost, s->stream));
-  CK(cudaMemcpyAsync(s->h_pin_out + (size_t)N * 25, s->d_reward, sizeof(float) * N, cudaMemcpyDeviceToHost, s->stream));
-  CK(cudaMemcpyAsync(s->h_pin_out + (size_t)N * 26, s->d_done, sizeof(float) * N, cudaMemcpyDeviceToHost, s->stream));
-  CK(cudaMemcpyAsync(s->h_pin_out + (size_t)N * 27, s->d_info, sizeof(float) * N * 4, cudaMemcpyDeviceToHost, s->stream));
-#else
-  memcpy(s->h_pin_out, s->d_obs, sizeof(float) * N * 25); memcpy(s->h_pin_out + (size_t)N * 25, s->d_reward, sizeof(float) * N);
-  memcpy(s->h_pin_out + (size_t)N * 26, s->d_done, sizeof(float) * N); memcpy(s->h_pin_out + (size_t)N * 27, s->d_info, sizeof(float) * N * 4);
-#endif
-  return 0;
+  return host_begin(s, TASK_FEEDING, false, action);
 }
 int ag_feeding_step_host_end(AgSim* s, float* obs, float* reward, float* done, float* info) {
   DevGuard guard__(s->device);
-  if (!s->feeding) return fail("ag_feeding_init not called");
-  const int N = s->S.N;
-#ifndef AG_CPU_EMU
-  CK(cudaStreamSynchronize(s->stream));
-  CK(cudaGetLastError());
-#endif
-  memcpy(obs, s->h_pin_out, sizeof(float) * N * 25);
-  memcpy(reward, s->h_pin_out + (size_t)N * 25, sizeof(float) * N);
-  memcpy(done, s->h_pin_out + (size_t)N * 26, sizeof(float) * N);
-  if (info) memcpy(info, s->h_pin_out + (size_t)N * 27, sizeof(float) * N * 4);
-  return 0;
-}
-int ag_feeding_step_host(AgSim* s, const float* action, float* obs, float* reward, float* done, float* info) {
-  if (ag_feeding_step_host_begin(s, action)) return -1;
-  return ag_feeding_step_host_end(s, obs, reward, done, info);
+  return host_end(s, TASK_FEEDING, false, StepOut{obs, nullptr, reward, done, info});
 }
 
 // ------------------------------------------------------------------ fused BedBathingEnv path
@@ -1643,7 +1680,7 @@ int ag_bathing_init(AgSim* s, const AgBathingParams* p, const int32_t* gender_is
   const int N = s->S.N;
   BathDev& B = s->B;
   B.P = *p;
-  drop_graph(s, 1);
+  drop_task_graphs(s, TASK_BATHING);
   const int T = p->n_targets_max;
   if (T <= 0 || T > 4096) return fail("bad target count");
   for (int j = 0; j < 7; j++) if (p->arm_links[j] < 0 || p->arm_links[j] >= s->nl) return fail("bad link");
@@ -1654,16 +1691,9 @@ int ag_bathing_init(AgSim* s, const AgBathingParams* p, const int32_t* gender_is
     B.targets = dalloc<float>(s, (size_t)T * 3 * N); B.alive = dalloc<int>(s, (size_t)T * N);
     B.n_slots = p->human_ncol_m > p->human_ncol_f ? p->human_ncol_m : p->human_ncol_f;
     B.dist_part = dalloc<float>(s, (size_t)(B.n_slots > 0 ? B.n_slots : 1) * N);
-    s->d_baction = dalloc<float>(s, (size_t)N * 7); s->d_bobs = dalloc<float>(s, (size_t)N * 24);
-    s->d_breward = dalloc<float>(s, N); s->d_bdone = dalloc<float>(s, N); s->d_binfo = dalloc<float>(s, (size_t)N * 4);
     s->B_dev = dalloc<BathDev>(s, 1);
-    if (!s->B_dev || !s->d_binfo || !B.dist_part) return fail("device allocation failed");
-#ifndef AG_CPU_EMU
-    CK(cudaMallocHost((void**)&s->h_bpin_in, sizeof(float) * N * 7));
-    CK(cudaMallocHost((void**)&s->h_bpin_out, sizeof(float) * N * 30));
-#else
-    s->h_bpin_in = (float*)malloc(sizeof(float) * N * 7); s->h_bpin_out = (float*)malloc(sizeof(float) * N * 30);
-#endif
+    if (!s->B_dev || !B.dist_part) return fail("device allocation failed");
+    if (io_alloc(s, s->io[TASK_BATHING], 7, ROBOT_OBS_W[TASK_BATHING], 0)) return -1;
   } else if (T != s->B.P.n_targets_max) return fail("target count changed");
   std::vector<float> tw((size_t)T * 3 * N); std::vector<int> al((size_t)T * N), tot(N, 0), zero(N, 0);
   for (int e = 0; e < N; e++)
@@ -1704,82 +1734,26 @@ int ag_bathing_set_target_frames(AgSim* s, const int32_t* link, const float* loc
   s->bath_frames = true;
   return 0;
 }
-static int bathing_step_enqueue(AgSim* s, const float* action_dev, float* obs, float* reward, float* done, float* info) {
-  const int N = s->S.N;
-  KP p = kp0(); p.p0 = action_dev; p.p1 = s->B_dev;
-  LAUNCH(s, k_bath_pre, N, p);
-  for (int i = 0; i < s->B.P.frame_skip * (s->cfg.num_substeps > 0 ? s->cfg.num_substeps : 1); i++) substep(s);
-  KP z = kp0();
-  LAUNCH(s, k_fk, (size_t)s->S.nb * N, z);
-  KP a = kp0(); a.p0 = s->S.movcol; a.i0 = s->S.nmovcol;
-  LAUNCH(s, k_aabb, (size_t)s->S.nmovcol * N, a);
-  KP l = kp0(); l.p0 = s->S.movlink; l.i0 = s->S.nmovlink;
-  LAUNCH(s, k_linkaabb, (size_t)s->S.nmovlink * N, l);
-  KP d = kp0(); d.p1 = s->B_dev;
-  LAUNCH(s, k_bath_dist, (size_t)N * s->B.n_slots, d);
-  KP q = kp0(); q.p0 = action_dev; q.p1 = s->B_dev; q.p2 = obs; q.p3 = reward; q.p4 = done; q.p5 = info;
-  LAUNCH(s, k_bath_post, N, q);
-  return 0;
-}
 int ag_bathing_step_dev(AgSim* s, const float* action_dev, float* obs_dev, float* reward_dev, float* done_dev, float* info_dev) {
   DevGuard guard__(s->device);
-  if (!s->bathing) return fail("ag_bathing_init not called");
-  int rc = run_step(s, 1, bathing_step_enqueue, action_dev, obs_dev, reward_dev, done_dev, info_dev);
-#ifndef AG_CPU_EMU
-  CK(cudaGetLastError());
-#endif
-  return rc;
+  return step_dev(s, TASK_BATHING, false, action_dev, StepOut{obs_dev, nullptr, reward_dev, done_dev, info_dev});
 }
 int ag_bathing_step_host(AgSim* s, const float* action, float* obs, float* reward, float* done, float* info) {
   DevGuard guard__(s->device);
-  if (!s->bathing) return fail("ag_bathing_init not called");
-  const int N = s->S.N;
-  memcpy(s->h_bpin_in, action, sizeof(float) * N * 7);
-#ifndef AG_CPU_EMU
-  CK(cudaMemcpyAsync(s->d_baction, s->h_bpin_in, sizeof(float) * N * 7, cudaMemcpyHostToDevice, s->stream));
-#else
-  memcpy(s->d_baction, s->h_bpin_in, sizeof(float) * N * 7);
-#endif
-  if (run_step(s, 1, bathing_step_enqueue, s->d_baction, s->d_bobs, s->d_breward, s->d_bdone, s->d_binfo)) return -1;
-#ifndef AG_CPU_EMU
-  CK(cudaMemcpyAsync(s->h_bpin_out, s->d_bobs, sizeof(float) * N * 24, cudaMemcpyDeviceToHost, s->stream));
-  CK(cudaMemcpyAsync(s->h_bpin_out + (size_t)N * 24, s->d_breward, sizeof(float) * N, cudaMemcpyDeviceToHost, s->stream));
-  CK(cudaMemcpyAsync(s->h_bpin_out + (size_t)N * 25, s->d_bdone, sizeof(float) * N, cudaMemcpyDeviceToHost, s->stream));
-  CK(cudaMemcpyAsync(s->h_bpin_out + (size_t)N * 26, s->d_binfo, sizeof(float) * N * 4, cudaMemcpyDeviceToHost, s->stream));
-  CK(cudaStreamSynchronize(s->stream));
-  CK(cudaGetLastError());
-#else
-  memcpy(s->h_bpin_out, s->d_bobs, sizeof(float) * N * 24); memcpy(s->h_bpin_out + (size_t)N * 24, s->d_breward, sizeof(float) * N);
-  memcpy(s->h_bpin_out + (size_t)N * 25, s->d_bdone, sizeof(float) * N); memcpy(s->h_bpin_out + (size_t)N * 26, s->d_binfo, sizeof(float) * N * 4);
-#endif
-  memcpy(obs, s->h_bpin_out, sizeof(float) * N * 24);
-  memcpy(reward, s->h_bpin_out + (size_t)N * 24, sizeof(float) * N);
-  memcpy(done, s->h_bpin_out + (size_t)N * 25, sizeof(float) * N);
-  if (info) memcpy(info, s->h_bpin_out + (size_t)N * 26, sizeof(float) * N * 4);
-  return 0;
+  return host_step(s, TASK_BATHING, false, action, StepOut{obs, nullptr, reward, done, info});
 }
 
 // ------------------------------------------------------------------ fused co-optimisation path (ag_coop.cuh)
-static size_t coop_smem_bytes(bool mlp) { return mlp ? (size_t)(AG_MLP_FLOATS + 2 * AG_MLP_H * AG_COOP_T) * sizeof(float) : 0; }
-
 int ag_coop_init(AgSim* s, const AgCoopParams* p, const double* limit_scale, const float* mlp) {
   DevGuard guard__(s->device);
   const int N = s->S.N;
   if (!p) return fail("ag_coop_init: bad arguments");
-  if (p->task == 0) {
-    if (!s->feeding) return fail("ag_coop_init: call ag_feeding_init first");
-    if (p->n_ctrl != 4) return fail("ag_coop_init: the feeding person has 4 controllable joints");
-  } else if (p->task == 1) {
-    if (!s->scratch) return fail("ag_coop_init: call ag_scratch_init first");
-    if (p->n_ctrl != 10) return fail("ag_coop_init: the scratch-itch person has 10 controllable joints");
-  } else if (p->task == 2) {
-    if (!s->bathing) return fail("ag_coop_init: call ag_bathing_init first");
-    if (!s->bath_frames) return fail("ag_coop_init: call ag_bathing_set_target_frames first");
-    if (p->n_ctrl != 10) return fail("ag_coop_init: the bed-bathing person has 10 controllable joints");
-  } else if (p->task == 3) {
-    if (!s->dressing) return fail("ag_coop_init: call ag_dressing_init first");
-    if (p->n_ctrl != 10) return fail("ag_coop_init: the dressing person has 10 controllable joints");
-  } else return fail("ag_coop_init: task must be 0 (feeding), 1 (scratch itch), 2 (bed bathing) or 3 (dressing)");
+  if (p->task < 0 || p->task > 3) return fail("ag_coop_init: task must be 0 (feeding), 1 (scratch itch), 2 (bed bathing) or 3 (dressing)");
+  const Task task = (Task)p->task;
+  if (!task_ready(s, task)) return fail(std::string("ag_coop_init: call ") + TASK_INIT[task] + " first");
+  if (task == TASK_BATHING && !s->bath_frames) return fail("ag_coop_init: call ag_bathing_set_target_frames first");
+  if (task == TASK_FEEDING && p->n_ctrl != 4) return fail("ag_coop_init: the feeding person has 4 controllable joints");
+  if (task != TASK_FEEDING && p->n_ctrl != 10) return fail("ag_coop_init: the person has 10 controllable joints");
   if (p->human_body_m < 0 || p->human_body_m >= s->nb || p->human_body_f < 0 || p->human_body_f >= s->nb) return fail("ag_coop_init: bad body");
   if (p->n_joints < 1 || p->n_joints > AG_COOP_MAXJ) return fail("ag_coop_init: 1..48 joints");
   for (int j = 0; j < p->n_joints; j++) {
@@ -1800,24 +1774,24 @@ int ag_coop_init(AgSim* s, const AgCoopParams* p, const double* limit_scale, con
     if (!(limit_scale[e] > 0.0 && limit_scale[e] <= 1.0)) return fail("ag_coop_init: limit_scale must be in (0, 1]");
     sc[e] = limit_scale[e];
   }
-  drop_graph(s, 4);
+  drop_graph(s->io[IO_COOP]);
   CoopDev& C = s->CO;
+  StepIO& io = s->io[IO_COOP];
   if (!s->coop) {             // buffers are allocated once; a later init (episode reset) only refreshes their contents
     C.limit_scale = dalloc<double>(s, N); C.prev_pose = dalloc<float>(s, (size_t)4 * N);
     C.mlp = dalloc<float>(s, AG_MLP_FLOATS);
-    s->d_caction = dalloc<float>(s, (size_t)N * (7 + AG_COOP_MAXC));
-    s->d_cobs_r = dalloc<float>(s, (size_t)N * 30); s->d_cobs_h = dalloc<float>(s, (size_t)N * 34);
-    s->d_creward = dalloc<float>(s, N); s->d_cdone = dalloc<float>(s, N); s->d_cinfo = dalloc<float>(s, (size_t)N * 4);
     s->CO_dev = dalloc<CoopDev>(s, 1);
-    if (!s->d_cinfo || !s->CO_dev) return fail("device allocation failed");
+    if (!s->CO_dev) return fail("device allocation failed");
+    // room for every task's widths; each init sets its own task's below
+    if (io_alloc(s, io, 7 + AG_COOP_MAXC, *std::max_element(ROBOT_OBS_W, ROBOT_OBS_W + 4), *std::max_element(HUMAN_OBS_W, HUMAN_OBS_W + 4))) return -1;
 #ifndef AG_CPU_EMU
     CK(cudaFuncSetAttribute(k_coop_limits, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)coop_smem_bytes(true)));
     CK(cudaFuncSetAttribute(k_coop_classify, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)coop_smem_bytes(true)));
 #endif
   }
   C.P = *p;
-  C.frame_skip = p->task == 0 ? s->F.P.frame_skip : (p->task == 1 ? s->SD.P.frame_skip : (p->task == 2 ? s->B.P.frame_skip : s->DP.D.P.frame_skip));
-  C.male = p->task == 0 ? s->F.male : (p->task == 1 ? s->SD.male : (p->task == 2 ? s->B.male : s->DP.D.male));
+  C.frame_skip = task_frame_skip(s, task);
+  C.male = task_male(s, task);
   C.mlp_on = mlp != nullptr;
   std::vector<float> none((size_t)4 * N, nanf(""));
   if (h2d(s, C.limit_scale, sc.data(), sizeof(double) * N) || h2d(s, C.prev_pose, none.data(), sizeof(float) * 4 * N)) return -1;
@@ -1831,92 +1805,17 @@ int ag_coop_init(AgSim* s, const AgCoopParams* p, const double* limit_scale, con
       kp.push_back(p->motor_gain); kd.push_back(1.f); mf.push_back(p->motor_force);
     }
   if (ag_set_motor_host(s, (int)links.size(), links.data(), 1, nullptr, kp.data(), kd.data(), mf.data())) return -1;
-  s->coop_width = 7 + p->n_ctrl;
+  io.act_w = 7 + p->n_ctrl; io.obs_w = ROBOT_OBS_W[task]; io.obs_h_w = HUMAN_OBS_W[task];
   s->coop = true;
-  return 0;
-}
-static void coop_limits_launch(AgSim* s) {
-  KP p = kp0(); p.n = s->S.N; p.p1 = s->CO_dev;
-#ifndef AG_CPU_EMU
-  int ps = s->profiling ? prof_slot(s, "k_coop_limits") : -1;
-  if (ps >= 0) prof_mark(s, ps, true);
-  k_coop_limits<<<(p.n + AG_COOP_T - 1) / AG_COOP_T, AG_COOP_T, coop_smem_bytes(s->CO.mlp_on), s->stream>>>(s->S, p);
-  if (ps >= 0) prof_mark(s, ps, false);
-#else
-  k_coop_limits(s->S, p);
-#endif
-  s->launches++;
-}
-static int coop_step_enqueue(AgSim* s, const float* action_dev, float* obs, float* reward, float* done, float* info) {
-  const int N = s->S.N, k = s->CO.P.n_ctrl, task = s->CO.P.task;
-  void* const task_devs[4] = {s->F_dev, s->SD_dev, s->B_dev, s->DP_dev};
-  void* task_dev = task_devs[task];
-  KP p = kp0(); p.p0 = action_dev; p.p1 = task_dev; p.i0 = k;
-  if (task == 0) LAUNCH(s, k_feed_pre, N, p); else if (task == 1) LAUNCH(s, k_scratch_pre, N, p);
-  else if (task == 2) LAUNCH(s, k_bath_pre, N, p); else LAUNCH(s, k_dress_pre, N, p);
-  KP c = kp0(); c.p0 = action_dev; c.p1 = s->CO_dev;
-  LAUNCH(s, k_coop_pre, N, c);
-  const int sub = s->cfg.num_substeps > 0 ? s->cfg.num_substeps : 1;
-  KP z = kp0();
-  for (int f = 0; f < s->CO.frame_skip; f++) {         // stepSimulation, then the person's limits (env.py:223-231)
-    for (int i = 0; i < sub; i++) substep(s);          // with a cloth, the last one launches k_cloth
-    coop_limits_launch(s);
-    if (task == 3) {     // then update_targets (dressing.py:210): the gown's anchor goes to the end effector
-      LAUNCH(s, k_fk, (size_t)s->S.nb * N, z);         // k_coop_limits' restored poses are what the next cloth snapshot sees
-      KP a = kp0(); a.p0 = s->C_dev; a.i0 = s->DP.D.P.ee_link;
-      LAUNCH(s, k_cloth_follow, N, a);
-    }
-  }
-  if (task != 3) LAUNCH(s, k_fk, (size_t)s->S.nb * N, z);
-  KP q = kp0(); q.p0 = action_dev; q.p1 = task_dev; q.p2 = obs; q.p3 = reward; q.p4 = done; q.p5 = info; q.i0 = k;
-  if (task == 0 || task == 2) {
-    KP a = kp0(); a.p0 = s->S.movcol; a.i0 = s->S.nmovcol;
-    LAUNCH(s, k_aabb, (size_t)s->S.nmovcol * N, a);
-    KP l = kp0(); l.p0 = s->S.movlink; l.i0 = s->S.nmovlink;
-    LAUNCH(s, k_linkaabb, (size_t)s->S.nmovlink * N, l);
-  }
-  if (task == 0) {
-    KP f = kp0(); f.p1 = s->F_dev;
-    LAUNCH(s, k_feed_food, (size_t)N * s->F.P.n_foods, f);
-    LAUNCH(s, k_feed_post, N, q);
-  } else if (task == 1) {
-    LAUNCH(s, k_scratch_post, N, q);
-  } else if (task == 3) {
-    LAUNCH(s, k_dress_post, N, q);
-  } else {             // the targets follow the arm (update_targets), with k_coop_limits' restorations in the final poses
-    KP t = kp0(); t.p1 = s->B_dev;
-    LAUNCH(s, k_bath_track, (size_t)N * s->B.P.n_targets_max, t);
-    KP d = kp0(); d.p1 = s->B_dev;
-    LAUNCH(s, k_bath_dist, (size_t)N * s->B.n_slots, d);
-    LAUNCH(s, k_bath_post, N, q);
-  }
-  KP o = kp0(); o.p1 = s->CO_dev; o.p2 = task_dev; o.p3 = s->coop_obs_h; o.p4 = info;
-  LAUNCH(s, k_coop_obs, N, o);
   return 0;
 }
 int ag_coop_step_dev(AgSim* s, const float* action_dev, float* obs_robot_dev, float* obs_human_dev, float* reward_dev, float* done_dev, float* info_dev) {
   DevGuard guard__(s->device);
-  if (!s->coop) return fail("ag_coop_init not called");
-  if (s->CO.P.task == 2 && !s->bath_frames) return fail("ag_coop_step: call ag_bathing_set_target_frames after ag_bathing_init");
-  if (s->CO.P.task == 3 && s->cloth_sub != 0) return fail("ag_coop_step: a stepSimulation is half done (ag_step with a partial substep count?)");
-  if (obs_human_dev != s->coop_obs_h) { drop_graph(s, 4); s->coop_obs_h = obs_human_dev; }
-  int rc = run_step(s, 4, coop_step_enqueue, action_dev, obs_robot_dev, reward_dev, done_dev, info_dev);
-#ifndef AG_CPU_EMU
-  CK(cudaGetLastError());
-#endif
-  return rc;
+  return step_dev(s, (Task)s->CO.P.task, true, action_dev, StepOut{obs_robot_dev, obs_human_dev, reward_dev, done_dev, info_dev});
 }
 int ag_coop_step_host(AgSim* s, const float* action, float* obs_robot, float* obs_human, float* reward, float* done, float* info) {
   DevGuard guard__(s->device);
-  if (!s->coop) return fail("ag_coop_init not called");
-  const int N = s->S.N;
-  static const size_t ro_of[4] = {25, 30, 24, 24}, ho_of[4] = {23, 34, 28, 28};
-  const size_t ro = ro_of[s->CO.P.task], ho = ho_of[s->CO.P.task];
-  if (h2d(s, s->d_caction, action, sizeof(float) * N * s->coop_width)) return -1;
-  if (ag_coop_step_dev(s, s->d_caction, s->d_cobs_r, s->d_cobs_h, s->d_creward, s->d_cdone, s->d_cinfo)) return -1;
-  if (d2h(s, obs_robot, s->d_cobs_r, sizeof(float) * N * ro) || d2h(s, obs_human, s->d_cobs_h, sizeof(float) * N * ho) ||
-      d2h(s, reward, s->d_creward, sizeof(float) * N) || d2h(s, done, s->d_cdone, sizeof(float) * N)) return -1;
-  return info ? d2h(s, info, s->d_cinfo, sizeof(float) * N * 4) : 0;
+  return host_step(s, (Task)s->CO.P.task, true, action, StepOut{obs_robot, obs_human, reward, done, info});
 }
 int ag_coop_classify(AgSim* s, int n, const float* x, float* p) {
   DevGuard guard__(s->device);

@@ -28,6 +28,11 @@ def _i32(a):
     return None if a is None else np.ascontiguousarray(a, dtype=np.int32)
 
 
+# floats per env of the robot's and the person's observation of each fused task, in AgCoopParams.task order
+_OBS_W = {'feeding': (25, 23), 'scratch': (30, 34), 'bathing': (24, 28), 'dressing': (24, 28)}
+_TASKS = tuple(_OBS_W)
+
+
 class BatchSim:
     def __init__(self, scene, cfg=None, n_envs=1, device=0, _lib=None):
         self.lib = _lib if _lib is not None else capi.load_library()
@@ -206,6 +211,22 @@ class BatchSim:
     def stream_ptr(self):
         return int(self.lib.ag_stream(self.h) or 0)
 
+    # ---- fused env steps: (robot obs, [person obs,] reward, done, info [n, 4]) of `task`, the person's with `coop`
+    def _step_outputs(self, task, coop):
+        ro, ho = _OBS_W[task]
+        obs = [np.zeros((self.n, ro), dtype=np.float32)] + ([np.zeros((self.n, ho), dtype=np.float32)] if coop else [])
+        return (*obs, np.zeros(self.n, dtype=np.float32), np.zeros(self.n, dtype=np.float32), np.zeros((self.n, 4), dtype=np.float32))
+
+    def _step_host(self, task, action, coop=False):
+        fn = self.lib.ag_coop_step_host if coop else getattr(self.lib, 'ag_%s_step_host' % task)
+        width = 7 + (int(self._coop_params.n_ctrl) if coop else 0)
+        out = self._step_outputs(task, coop)
+        self._ck(fn(self.h, _p(_f32(action, (self.n, width))), *map(_p, out)))
+        return out
+
+    def _step_dev(self, fn, *ptrs):
+        self._ck(fn(self.h, *[C.c_void_p(p) for p in ptrs]))
+
     # ---- fused feeding path
     def feeding_init(self, params, gender_is_male):
         self._feed_params = params
@@ -244,15 +265,10 @@ class BatchSim:
         self._ck(self.lib.ag_bathing_set_target_frames(self.h, _p(lk), _p(_f32(local, (self.n, T, 3)))))
 
     def bathing_step_host(self, action):
-        a = _f32(action, (self.n, 7))
-        obs = np.zeros((self.n, 24), dtype=np.float32)
-        rew, done = np.zeros(self.n, dtype=np.float32), np.zeros(self.n, dtype=np.float32)
-        info = np.zeros((self.n, 4), dtype=np.float32)
-        self._ck(self.lib.ag_bathing_step_host(self.h, _p(a), _p(obs), _p(rew), _p(done), _p(info)))
-        return obs, rew, done, info
+        return self._step_host('bathing', action)
 
     def bathing_step_dev(self, action_ptr, obs_ptr, reward_ptr, done_ptr, info_ptr):
-        self._ck(self.lib.ag_bathing_step_dev(self.h, C.c_void_p(action_ptr), C.c_void_p(obs_ptr), C.c_void_p(reward_ptr), C.c_void_p(done_ptr), C.c_void_p(info_ptr)))
+        self._step_dev(self.lib.ag_bathing_step_dev, action_ptr, obs_ptr, reward_ptr, done_ptr, info_ptr)
 
     # ---- cloth (ag_cloth_*; node arrays in the PUBLIC node order of the ClothModel)
     def cloth_init(self, model, col_links, col_static, anchor_nodes, anchor_local, gravity=(0, 0, -9.81), max_contacts=1024):
@@ -300,39 +316,25 @@ class BatchSim:
         self._ck(self.lib.ag_scratch_init(self.h, C.byref(params), _p(_i32(gender_is_male)), _p(_i32(limb_link)), _p(_f32(target_local, (self.n, 3)))))
 
     def scratch_step_host(self, action):
-        a = _f32(action, (self.n, 7))
-        obs = np.empty((self.n, 30), dtype=np.float32)
-        rew = np.empty(self.n, dtype=np.float32)
-        done = np.empty(self.n, dtype=np.float32)
-        info = np.empty((self.n, 4), dtype=np.float32)
-        self._ck(self.lib.ag_scratch_step_host(self.h, _p(a), _p(obs), _p(rew), _p(done), _p(info)))
-        return obs, rew, done, info
+        return self._step_host('scratch', action)
 
     def scratch_step_dev(self, action_ptr, obs_ptr, reward_ptr, done_ptr, info_ptr):
-        self._ck(self.lib.ag_scratch_step_dev(self.h, action_ptr, obs_ptr, reward_ptr, done_ptr, info_ptr))
+        self._step_dev(self.lib.ag_scratch_step_dev, action_ptr, obs_ptr, reward_ptr, done_ptr, info_ptr)
 
     # ---- fused co-optimisation path (the person's half; call after feeding_init / scratch_init / bathing_init / dressing_init)
     def coop_init(self, params, limit_scale=None, mlp=None):
         """limit_scale [n] or None; mlp: the packed classifier weights (fp32, agphys.h order) or None"""
         self._coop_params = params
-        self._coop_dims = {0: (25, 23), 1: (30, 34), 2: (24, 28), 3: (24, 28)}.get(int(params.task), (0, 0))
         ls = None if limit_scale is None else np.ascontiguousarray(np.broadcast_to(np.asarray(limit_scale, dtype=np.float64), (self.n,)))
         w = None if mlp is None else np.ascontiguousarray(mlp, dtype=np.float32)
         self._ck(self.lib.ag_coop_init(self.h, C.byref(params), _p(ls), _p(w)))
 
     def coop_step_host(self, action):
         """action [n, 7 + n_ctrl] (robot, then person) -> obs_robot, obs_human, reward, done, info [n, 4]"""
-        a = _f32(action, (self.n, 7 + int(self._coop_params.n_ctrl)))
-        ro, ho = self._coop_dims
-        obs_r, obs_h = np.empty((self.n, ro), dtype=np.float32), np.empty((self.n, ho), dtype=np.float32)
-        rew, done = np.empty(self.n, dtype=np.float32), np.empty(self.n, dtype=np.float32)
-        info = np.empty((self.n, 4), dtype=np.float32)
-        self._ck(self.lib.ag_coop_step_host(self.h, _p(a), _p(obs_r), _p(obs_h), _p(rew), _p(done), _p(info)))
-        return obs_r, obs_h, rew, done, info
+        return self._step_host(_TASKS[int(self._coop_params.task)], action, coop=True)
 
     def coop_step_dev(self, action_ptr, obs_robot_ptr, obs_human_ptr, reward_ptr, done_ptr, info_ptr):
-        self._ck(self.lib.ag_coop_step_dev(self.h, C.c_void_p(action_ptr), C.c_void_p(obs_robot_ptr), C.c_void_p(obs_human_ptr),
-                                           C.c_void_p(reward_ptr), C.c_void_p(done_ptr), C.c_void_p(info_ptr)))
+        self._step_dev(self.lib.ag_coop_step_dev, action_ptr, obs_robot_ptr, obs_human_ptr, reward_ptr, done_ptr, info_ptr)
 
     def coop_classify(self, x):
         """the device joint-limit classifier on x [m, 4] -> p [m]"""
@@ -364,42 +366,27 @@ class BatchSim:
         self._ck(self.lib.ag_dressing_reset_episode(self.h, _p(_i32(mask))))
 
     def dressing_step_host(self, action):
-        a = _f32(action, (self.n, 7))
-        obs = np.empty((self.n, 24), dtype=np.float32)
-        rew = np.empty(self.n, dtype=np.float32)
-        done = np.empty(self.n, dtype=np.float32)
-        info = np.empty((self.n, 4), dtype=np.float32)
-        self._ck(self.lib.ag_dressing_step_host(self.h, _p(a), _p(obs), _p(rew), _p(done), _p(info)))
-        return obs, rew, done, info
+        return self._step_host('dressing', action)
 
     def dressing_step_dev(self, action_ptr, obs_ptr, reward_ptr, done_ptr, info_ptr):
-        self._ck(self.lib.ag_dressing_step_dev(self.h, action_ptr, obs_ptr, reward_ptr, done_ptr, info_ptr))
+        self._step_dev(self.lib.ag_dressing_step_dev, action_ptr, obs_ptr, reward_ptr, done_ptr, info_ptr)
 
     def feeding_reset_episode(self, mask=None):
         self._ck(self.lib.ag_feeding_reset_episode(self.h, _p(_i32(mask))))
 
     def feeding_step_host(self, action):
-        a = _f32(action, (self.n, 7))
-        obs = np.zeros((self.n, 25), dtype=np.float32)
-        rew, done = np.zeros(self.n, dtype=np.float32), np.zeros(self.n, dtype=np.float32)
-        info = np.zeros((self.n, 4), dtype=np.float32)
-        self._ck(self.lib.ag_feeding_step_host(self.h, _p(a), _p(obs), _p(rew), _p(done), _p(info)))
-        return obs, rew, done, info
+        return self._step_host('feeding', action)
 
     def feeding_step_host_begin(self, action):
-        self._host_a = _f32(action, (self.n, 7))
-        self._ck(self.lib.ag_feeding_step_host_begin(self.h, _p(self._host_a)))
+        self._ck(self.lib.ag_feeding_step_host_begin(self.h, _p(_f32(action, (self.n, 7)))))
 
     def feeding_step_host_end(self):
-        obs = np.zeros((self.n, 25), dtype=np.float32)
-        rew, done = np.zeros(self.n, dtype=np.float32), np.zeros(self.n, dtype=np.float32)
-        info = np.zeros((self.n, 4), dtype=np.float32)
-        self._ck(self.lib.ag_feeding_step_host_end(self.h, _p(obs), _p(rew), _p(done), _p(info)))
-        return obs, rew, done, info
+        out = self._step_outputs('feeding', False)
+        self._ck(self.lib.ag_feeding_step_host_end(self.h, *map(_p, out)))
+        return out
 
     def feeding_step_dev(self, action_ptr, obs_ptr, reward_ptr, done_ptr, info_ptr):
-        self._ck(self.lib.ag_feeding_step_dev(self.h, C.c_void_p(action_ptr), C.c_void_p(obs_ptr), C.c_void_p(reward_ptr),
-                                              C.c_void_p(done_ptr), C.c_void_p(info_ptr)))
+        self._step_dev(self.lib.ag_feeding_step_dev, action_ptr, obs_ptr, reward_ptr, done_ptr, info_ptr)
 
 
 class BatchSimGroup:

@@ -13,7 +13,8 @@
  *   - Batched buffers are env-major: element (env e, item i, component c) of a [N][K][C] buffer is
  *     at ((e*K)+i)*C + c.  `*_host` calls take host pointers and include the H2D/D2H copies;
  *     `*_dev` calls take device pointers valid on the simulation's device and enqueue on the
- *     simulation's stream.
+ *     simulation's stream.  The fused env steps' host-buffer calls (`*_step_host`, `*_step_host_end`)
+ *     accept a NULL `info`.
  *   - Quaternions are [x,y,z,w] (reference agents/agent.py:60, env.py:192).
  *   - Link index == joint index == DFS pre-order over the URDF tree, base = -1 (reference
  *     agents/jaco.py:8-18).  In this ABI links are addressed by *global link id* (int) obtained from
@@ -214,7 +215,7 @@ int ag_feeding_reset_episode(AgSim* sim, const int32_t* env_mask);
 int ag_feeding_set_tremor(AgSim* sim, const int32_t* on, const float* rest, const float* amplitude);
 int ag_feeding_step_dev(AgSim* sim, const float* action_dev, float* obs_dev, float* reward_dev,
                         float* done_dev, float* info_dev);
-/* host-buffer variant (pinned or pageable): H2D of action, D2H of obs/reward/done/info inside */
+/* host-buffer variant (pinned or pageable): H2D of action, D2H of obs/reward/done/info inside; info may be NULL */
 int ag_feeding_step_host(AgSim* sim, const float* action, float* obs, float* reward, float* done, float* info);
 /* the same in two halves, so that several sims (sub-batches on their own streams) overlap: `begin` stages the actions and
  * enqueues H2D + step + D2H on the sim's stream and returns, `end` waits for the stream and hands the results out */
