@@ -92,6 +92,18 @@ class AgScratchParams(C.Structure):
                 ('c_v', C.c_float), ('c_f', C.c_float), ('c_hf', C.c_float), ('task_success_threshold', C.c_float)]
 
 
+class AgDrinkingParams(C.Structure):
+    _fields_ = [('robot_body', C.c_int32), ('tool_body', C.c_int32), ('human_body_m', C.c_int32), ('human_body_f', C.c_int32),
+                ('arm_links', C.c_int32 * 7), ('ee_link', C.c_int32), ('head_link_m', C.c_int32), ('head_link_f', C.c_int32),
+                ('water_body0', C.c_int32), ('n_water', C.c_int32),
+                ('arm_lower', C.c_float * 7), ('arm_upper', C.c_float * 7), ('mouth_m', C.c_float * 3), ('mouth_f', C.c_float * 3),
+                ('cup_frame_pos', C.c_float * 3), ('cup_frame_quat', C.c_float * 4), ('cup_top', C.c_float * 3), ('cup_bottom', C.c_float * 3),
+                ('action_multiplier', C.c_float), ('frame_skip', C.c_int32),
+                ('w_distance', C.c_float), ('w_action', C.c_float), ('w_cup_tilt', C.c_float), ('w_drinking', C.c_float),
+                ('c_v', C.c_float), ('c_f', C.c_float), ('c_hf', C.c_float), ('c_fd', C.c_float), ('c_fdv', C.c_float),
+                ('task_success_threshold', C.c_float), ('seed', C.c_uint64)]
+
+
 AG_COOP_MAXJ, AG_COOP_MAXC = 48, 10
 
 
@@ -251,6 +263,10 @@ def load_library(path=None):
     lib.ag_scratch_init.argtypes = [vp, C.POINTER(AgScratchParams), vp, vp, vp]
     lib.ag_scratch_step_dev.argtypes = [vp, vp, vp, vp, vp, vp]
     lib.ag_scratch_step_host.argtypes = [vp, vp, vp, vp, vp, vp]
+    lib.ag_drinking_init.argtypes = [vp, C.POINTER(AgDrinkingParams), vp]
+    lib.ag_drinking_step_dev.argtypes = [vp, vp, vp, vp, vp, vp]
+    lib.ag_drinking_step_host.argtypes = [vp, vp, vp, vp, vp, vp]
+    lib.ag_drinking_get_state.argtypes = [vp, vp, vp, vp]
     lib.ag_coop_init.argtypes = [vp, C.POINTER(AgCoopParams), vp, vp]
     lib.ag_coop_step_dev.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     lib.ag_coop_step_host.argtypes = [vp, vp, vp, vp, vp, vp, vp]
@@ -287,4 +303,5 @@ EXPORTED_SYMBOLS = [
     'ag_cloth_get_contacts', 'ag_cloth_device_state', 'ag_scratch_init', 'ag_scratch_step_dev', 'ag_scratch_step_host', 'ag_render', 'ag_set_body_gravity', 'ag_get_link_aabb', 'ag_dressing_init', 'ag_dressing_reset_episode', 'ag_dressing_set_tremor', 'ag_set_motor_force_scale', 'ag_dressing_step_dev', 'ag_dressing_step_host',
     'ag_overflow_count', 'ag_get_solver_stats', 'ag_get_pgs_cycles', 'ag_get_pgs_trips', 'ag_get_pgs_occupancy', 'ag_profile_enable', 'ag_profile_get',
     'ag_coop_init', 'ag_coop_step_dev', 'ag_coop_step_host', 'ag_coop_classify', 'ag_bathing_set_target_frames',
+    'ag_drinking_init', 'ag_drinking_step_dev', 'ag_drinking_step_host', 'ag_drinking_get_state',
 ]

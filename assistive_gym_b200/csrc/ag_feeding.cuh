@@ -144,26 +144,35 @@ AG_HDN inline void closest_body(int e, const SimDev& S, const KP& p) {
 }
 
 // ------------------------------------------------------------------ fused FeedingEnv
-// action -> PD targets.  p0 = action [N][7 + i0] (env-major; the robot's 7 come first), p1 = FeedDev*
-AG_HDN inline void feeding_pre_body(int e, const SimDev& S, const KP& p) {
+// The robot's half of take_step (env.py:186-197) for a 7-joint arm: the raw action row is kept in `action` [7][N] (the reward's
+// action term), clipped to [-1, 1], scaled, accumulated frame_skip times inside the joint limits; the result is each joint's
+// PD target.  Feeding's and Drinking's pre kernels both call it.
+AG_HD void arm_action_targets(const SimDev& S, int e, const float* act, float* action, const int32_t* arm_links, const float* lower,
+                              const float* upper, float multiplier, int frame_skip) {
   const int N = S.N;
-  const FeedDev& F = *(const FeedDev*)p.p1;
-  const float* act = (const float*)p.p0 + (size_t)e * (7 + p.i0);
-  F.iteration[e] += 1;
   for (int j = 0; j < 7; j++) {
     float raw = act[j];
-    F.action[(size_t)j * N + e] = raw;
-    float a = clampf(raw, -1.f, 1.f) * F.P.action_multiplier;
-    int k = F.P.arm_links[j];
+    action[(size_t)j * N + e] = raw;
+    float a = clampf(raw, -1.f, 1.f) * multiplier;
+    int k = arm_links[j];
     float q = ld1(S.jq, k, N, e);
-    float lo = F.P.arm_lower[j], hi = F.P.arm_upper[j];
-    for (int s = 0; s < F.P.frame_skip; s++) {
+    float lo = lower[j], hi = upper[j];
+    for (int s = 0; s < frame_skip; s++) {
       if (q + a < lo) { a = 0.f; q = lo; }
       if (q + a > hi) { a = 0.f; q = hi; }
       q += a;
     }
     st1(S.motor_target, k, N, e, q);
   }
+}
+
+// action -> PD targets.  p0 = action [N][7 + i0] (env-major; the robot's 7 come first), p1 = FeedDev*
+AG_HDN inline void feeding_pre_body(int e, const SimDev& S, const KP& p) {
+  const int N = S.N;
+  const FeedDev& F = *(const FeedDev*)p.p1;
+  const float* act = (const float*)p.p0 + (size_t)e * (7 + p.i0);
+  F.iteration[e] += 1;
+  arm_action_targets(S, e, act, F.action, F.P.arm_links, F.P.arm_lower, F.P.arm_upper, F.P.action_multiplier, F.P.frame_skip);
   // tremor (env.py:212-215): the head joints are driven to rest +- amplitude, sign flips every env step
   if (F.tremor_on[e]) {
     bool male = F.male[e] != 0;

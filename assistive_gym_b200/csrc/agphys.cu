@@ -19,6 +19,7 @@
 #include "ag_render.cuh"
 #include "ag_scratch.cuh"
 #include "ag_coop.cuh"
+#include "ag_drinking.cuh"
 
 #ifndef AG_CPU_EMU
 #include <cuda_runtime.h>
@@ -112,6 +113,9 @@ AG_KERNEL(k_dress_pre, dressing_pre_body)
 AG_KERNEL(k_dress_post, dressing_post_body)
 AG_KERNEL(k_scratch_pre, scratch_pre_body)
 AG_KERNEL(k_scratch_post, scratch_post_body)
+AG_KERNEL(k_drink_pre, drinking_pre_body)
+AG_KERNEL(k_drink_water, drinking_water_body)
+AG_KERNEL(k_drink_post, drinking_post_body)
 AG_KERNEL(k_render, render_body)
 AG_KERNEL(k_cloth_snap, cloth_snap_body)
 AG_KERNEL(k_cloth_follow, cloth_follow_body)
@@ -161,11 +165,11 @@ static void k_coop_classify(SimDev, KP p) {
 
 // ------------------------------------------------------------------ host object
 // The fused tasks, numbered as AgCoopParams.task.  AgSim::io holds one record per task and, at IO_COOP, the
-// co-optimisation step's.
-enum Task { TASK_FEEDING = 0, TASK_SCRATCH = 1, TASK_BATHING = 2, TASK_DRESSING = 3 };
-static const int IO_COOP = 4;
-static const int ROBOT_OBS_W[4] = {25, 30, 24, 24}, HUMAN_OBS_W[4] = {23, 34, 28, 28};   // floats per env, by task
-static const char* const TASK_INIT[4] = {"ag_feeding_init", "ag_scratch_init", "ag_bathing_init", "ag_dressing_init"};
+// co-optimisation step's.  Drinking has no co-optimisation step yet (HUMAN_OBS_W 0).
+enum Task { TASK_FEEDING = 0, TASK_SCRATCH = 1, TASK_BATHING = 2, TASK_DRESSING = 3, TASK_DRINKING = 4 };
+static const int IO_COOP = 5;
+static const int ROBOT_OBS_W[5] = {25, 30, 24, 24, 25}, HUMAN_OBS_W[5] = {23, 34, 28, 28, 0};   // floats per env, by task
+static const char* const TASK_INIT[5] = {"ag_feeding_init", "ag_scratch_init", "ag_bathing_init", "ag_dressing_init", "ag_drinking_init"};
 
 // The outputs of one fused env step; obs_h (the person's observation) only for the co-optimisation step.
 struct StepOut { float *obs, *obs_h, *reward, *done, *info; };
@@ -201,11 +205,12 @@ struct AgSim {
   ClothDev C; ClothDev* C_dev; bool cloth; int cloth_sub, cloth_npt, cloth_qs;
   DressPost DP; DressPost* DP_dev; bool dressing;
   ScratchDev SD; ScratchDev* SD_dev; bool scratch;
+  DrinkDev DK; DrinkDev* DK_dev; bool drinking;
   size_t render_pix; int render_n; int* d_render_ids; unsigned char* d_render_rgba; float* d_render_depth; void* d_render_dev;
   // co-optimisation (the person's half; the robot's half is the task's state above)
   CoopDev CO; CoopDev* CO_dev; bool coop;
   // the fused-step entry points (Task, then IO_COOP); CUDA-graph replay of their steps
-  StepIO io[5];
+  StepIO io[6];
   bool use_graph; int graph_failures;
   // profiling
   bool profiling;
@@ -370,7 +375,7 @@ AgSim* ag_create(const AgSceneDesc* d, const AgConfig* cfg, int n_envs, int devi
   AgSim* s = new AgSim();
   memset(&s->S, 0, sizeof(SimDev));
   memset(&s->F, 0, sizeof(FeedDev));
-  s->cfg = *cfg; s->device = device; s->launches = 0; s->feeding = false; s->bathing = false; s->cloth = false; s->cloth_sub = 0; s->C_dev = nullptr; s->dressing = false; s->DP_dev = nullptr; s->scratch = false; s->SD_dev = nullptr; s->render_pix = 0; s->render_n = 0; s->d_render_ids = nullptr; s->d_render_rgba = nullptr; s->d_render_depth = nullptr; s->d_render_dev = nullptr; s->use_graph = true; s->graph_failures = 0; s->coop = false; s->CO_dev = nullptr; s->B_dev = nullptr; s->stream = nullptr; s->F_dev = nullptr; s->profiling = false;
+  s->cfg = *cfg; s->device = device; s->launches = 0; s->feeding = false; s->bathing = false; s->cloth = false; s->cloth_sub = 0; s->C_dev = nullptr; s->dressing = false; s->DP_dev = nullptr; s->scratch = false; s->SD_dev = nullptr; s->drinking = false; s->DK_dev = nullptr; s->render_pix = 0; s->render_n = 0; s->d_render_ids = nullptr; s->d_render_rgba = nullptr; s->d_render_depth = nullptr; s->d_render_dev = nullptr; s->use_graph = true; s->graph_failures = 0; s->coop = false; s->CO_dev = nullptr; s->B_dev = nullptr; s->stream = nullptr; s->F_dev = nullptr; s->profiling = false;
   s->d_stage = nullptr; s->stage_floats = 0;
 #ifndef AG_CPU_EMU
   { int ndev = 0; if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) { g_err = "no such CUDA device (is a CUDA device present? there is no CPU fallback)"; delete s; return nullptr; } }
@@ -1065,6 +1070,7 @@ static bool task_ready(const AgSim* s, Task task) {
     case TASK_SCRATCH: return s->scratch;
     case TASK_BATHING: return s->bathing;
     case TASK_DRESSING: return s->dressing;
+    case TASK_DRINKING: return s->drinking;
   }
   return false;
 }
@@ -1074,6 +1080,7 @@ static void* task_dev(const AgSim* s, Task task) {
     case TASK_SCRATCH: return s->SD_dev;
     case TASK_BATHING: return s->B_dev;
     case TASK_DRESSING: return s->DP_dev;
+    case TASK_DRINKING: return s->DK_dev;
   }
   return nullptr;
 }
@@ -1083,6 +1090,7 @@ static int task_frame_skip(const AgSim* s, Task task) {
     case TASK_SCRATCH: return s->SD.P.frame_skip;
     case TASK_BATHING: return s->B.P.frame_skip;
     case TASK_DRESSING: return s->DP.D.P.frame_skip;
+    case TASK_DRINKING: return s->DK.P.frame_skip;
   }
   return 0;
 }
@@ -1092,6 +1100,7 @@ static int* task_male(const AgSim* s, Task task) {
     case TASK_SCRATCH: return s->SD.male;
     case TASK_BATHING: return s->B.male;
     case TASK_DRESSING: return s->DP.D.male;
+    case TASK_DRINKING: return s->DK.male;
   }
   return nullptr;
 }
@@ -1140,6 +1149,7 @@ static int fused_enqueue(AgSim* s, Task task, bool coop, const float* action, co
     case TASK_SCRATCH: LAUNCH(s, k_scratch_pre, N, p); break;
     case TASK_BATHING: LAUNCH(s, k_bath_pre, N, p); break;
     case TASK_DRESSING: LAUNCH(s, k_dress_pre, N, p); break;
+    case TASK_DRINKING: LAUNCH(s, k_drink_pre, N, p); break;
   }
   if (coop) {
     KP c = kp0(); c.p0 = action; c.p1 = s->CO_dev;
@@ -1158,7 +1168,7 @@ static int fused_enqueue(AgSim* s, Task task, bool coop, const float* action, co
     }
   }
   if (task != TASK_DRESSING) LAUNCH(s, k_fk, (size_t)s->S.nb * N, z);
-  if (task == TASK_FEEDING || task == TASK_BATHING) {
+  if (task == TASK_FEEDING || task == TASK_BATHING || task == TASK_DRINKING) {     // the boxes the near tests read
     KP a = kp0(); a.p0 = s->S.movcol; a.i0 = s->S.nmovcol;
     LAUNCH(s, k_aabb, (size_t)s->S.nmovcol * N, a);
     KP l = kp0(); l.p0 = s->S.movlink; l.i0 = s->S.nmovlink;
@@ -1178,6 +1188,10 @@ static int fused_enqueue(AgSim* s, Task task, bool coop, const float* action, co
       LAUNCH(s, k_bath_post, N, q);
       break;
     case TASK_DRESSING: LAUNCH(s, k_dress_post, N, q); break;
+    case TASK_DRINKING:
+      LAUNCH(s, k_drink_water, (size_t)N * s->DK.P.n_water, t);
+      LAUNCH(s, k_drink_post, N, q);
+      break;
   }
   if (coop) {
     KP h = kp0(); h.p1 = s->CO_dev; h.p2 = dev; h.p3 = o.obs_h; h.p4 = o.info;
@@ -1602,6 +1616,60 @@ int ag_scratch_step_host(AgSim* s, const float* action, float* obs, float* rewar
   return host_step(s, TASK_SCRATCH, false, action, StepOut{obs, nullptr, reward, done, info});
 }
 
+// ------------------------------------------------------------------ fused DrinkingEnv path (ag_drinking.cuh)
+int ag_drinking_init(AgSim* s, const AgDrinkingParams* p, const int32_t* gender_is_male) {
+  DevGuard guard__(s->device);
+  const int N = s->S.N;
+  if (!p || !gender_is_male) return fail("ag_drinking_init: bad arguments");
+  if (p->n_water < 1 || p->n_water > 64) return fail("ag_drinking_init: 1..64 water particles");
+  const int bodies[5] = {p->robot_body, p->tool_body, p->human_body_m, p->human_body_f, p->water_body0};
+  for (int b : bodies) if (b < 0 || b >= s->nb) return fail("ag_drinking_init: bad body");
+  if (p->water_body0 + p->n_water > s->nb) return fail("ag_drinking_init: bad body (the water particles run past the last body)");
+  for (int j = 0; j < 7; j++) if (p->arm_links[j] < 0 || p->arm_links[j] >= s->nl) return fail("ag_drinking_init: bad arm link");
+  if (p->ee_link < 0 || p->ee_link >= s->nl || p->head_link_m < 0 || p->head_link_m >= s->nl || p->head_link_f < 0 || p->head_link_f >= s->nl)
+    return fail("ag_drinking_init: bad link");
+  if (p->frame_skip < 0) return fail("ag_drinking_init: bad frame_skip");
+  DrinkDev& D = s->DK;
+  D.P = *p;
+  drop_task_graphs(s, TASK_DRINKING);    // the captured steps launch k_drink_water over the previous particle count
+  if (!s->drinking) {         // buffers are allocated once; a later init (episode reset) only refreshes their contents
+    D.male = dalloc<int>(s, N); D.iteration = dalloc<int>(s, N); D.task_success = dalloc<int>(s, N);
+    D.waters = dalloc<unsigned long long>(s, N); D.waters_active = dalloc<unsigned long long>(s, N); D.rng = dalloc<unsigned long long>(s, N);
+    D.status = dalloc<int>(s, (size_t)64 * N); D.action = dalloc<float>(s, (size_t)7 * N);
+    s->DK_dev = dalloc<DrinkDev>(s, 1);
+    if (!D.male || !D.iteration || !D.task_success || !D.waters || !D.waters_active || !D.rng || !D.status || !D.action || !s->DK_dev)
+      return fail("device allocation failed");
+    if (io_alloc(s, s->io[TASK_DRINKING], 7, ROBOT_OBS_W[TASK_DRINKING], 0)) return -1;
+  }
+  const unsigned long long full = p->n_water == 64 ? ~0ull : (1ull << p->n_water) - 1;
+  std::vector<unsigned long long> w(N, full), rng(N);
+  for (int e = 0; e < N; e++) rng[e] = (p->seed + 0x9E3779B97F4A7C15ull * (unsigned long long)(e + 1)) | 1ull;
+  if (h2d(s, D.male, gender_is_male, sizeof(int) * N) || h2d(s, D.waters, w.data(), sizeof(unsigned long long) * N) ||
+      h2d(s, D.waters_active, w.data(), sizeof(unsigned long long) * N) || h2d(s, D.rng, rng.data(), sizeof(unsigned long long) * N))
+    return -1;
+  if (dev_zero(s, D.iteration, sizeof(int) * N) || dev_zero(s, D.task_success, sizeof(int) * N)) return -1;
+  if (h2d(s, s->DK_dev, &D, sizeof(DrinkDev))) return fail("DrinkDev upload failed");
+  s->drinking = true;
+  return 0;
+}
+int ag_drinking_step_dev(AgSim* s, const float* action_dev, float* obs_dev, float* reward_dev, float* done_dev, float* info_dev) {
+  DevGuard guard__(s->device);
+  return step_dev(s, TASK_DRINKING, false, action_dev, StepOut{obs_dev, nullptr, reward_dev, done_dev, info_dev});
+}
+int ag_drinking_step_host(AgSim* s, const float* action, float* obs, float* reward, float* done, float* info) {
+  DevGuard guard__(s->device);
+  return host_step(s, TASK_DRINKING, false, action, StepOut{obs, nullptr, reward, done, info});
+}
+int ag_drinking_get_state(AgSim* s, int32_t* task_success, uint64_t* waters, uint64_t* waters_active) {
+  DevGuard guard__(s->device);
+  if (!s->drinking) return fail("ag_drinking_init not called");
+  const int N = s->S.N;
+  if (task_success && d2h(s, task_success, s->DK.task_success, sizeof(int) * N)) return -1;
+  if (waters && d2h(s, waters, s->DK.waters, sizeof(uint64_t) * N)) return -1;
+  if (waters_active && d2h(s, waters_active, s->DK.waters_active, sizeof(uint64_t) * N)) return -1;
+  return 0;
+}
+
 // ------------------------------------------------------------------ fused FeedingEnv path
 int ag_feeding_init(AgSim* s, const AgFeedingParams* p, const int32_t* gender_is_male) {
   DevGuard guard__(s->device);
@@ -1748,6 +1816,7 @@ int ag_coop_init(AgSim* s, const AgCoopParams* p, const double* limit_scale, con
   DevGuard guard__(s->device);
   const int N = s->S.N;
   if (!p) return fail("ag_coop_init: bad arguments");
+  if (p->task == TASK_DRINKING) return fail("ag_coop_init: task must be 0 (feeding), 1 (scratch itch), 2 (bed bathing) or 3 (dressing): the drinking co-optimisation id (task 4, DrinkingJacoHuman-v1) is not built yet");
   if (p->task < 0 || p->task > 3) return fail("ag_coop_init: task must be 0 (feeding), 1 (scratch itch), 2 (bed bathing) or 3 (dressing)");
   const Task task = (Task)p->task;
   if (!task_ready(s, task)) return fail(std::string("ag_coop_init: call ") + TASK_INIT[task] + " first");

@@ -6,12 +6,13 @@ env.py:114-134, `Human.init/setup_joints` human.py:72-127, `Tool.init` tool.py:1
 particles (4 x 4 x 4 spheres of radius 5 mm, 1 g) instead of 8 food particles; `numSubSteps = 4`, `numSolverIterations = 10`
 (drinking.py:157) are `config()`.
 
-Status: per-call API path only (no fused kernels, no bench line); checked on the CPU (oracle and host-compiled kernel bodies,
-tests/test_drinking.py, tests/test_reference_drinking_semantics.py); NOT run on a GPU in the round that added it."""
+Status: per-call API path (`DrinkingEnv.step`) and the fused device step (`start_fused`, `ag_drinking_step_*`, ag_drinking.cuh,
+`DrinkingEnv.step_fused`, `AssistiveVecEnv`); both replay the reference's own rollout (tests/test_reference_drinking_semantics.py,
+tests/test_drinking_fused.py), the fused step on the H100 too; its rate is tools/gpu_drinking_bench.py's."""
 import numpy as np
 
 from . import capi
-from .feeding_batch import HEAD_JOINTS, HUMAN_PRESET, IMPAIRMENTS, TREMOR_JOINTS, FeedingBatch
+from .feeding_batch import HEAD_JOINTS, HEAD_LINK, HUMAN_PRESET, IMPAIRMENTS, TREMOR_JOINTS, FeedingBatch
 from .human_model import create_human
 from .kinematics import BodyKinematics, q_from_rpy, q_mul, q_rot
 from .scene import SceneBuilder, quat_from_rpy
@@ -75,6 +76,45 @@ class DrinkingBatch(FeedingBatch):
     def config(**kw):
         """drinking.py:157: four substeps per stepSimulation, ten solver iterations; a contact budget for 64 particles in a cup."""
         return capi.default_config(**dict(dict(num_substeps=4, num_solver_iters=10, max_contacts=512), **kw))
+
+    def drinking_params(self, seed=1001):
+        """AgDrinkingParams of the fused step; the weights are the per-call env's (config.ini [drinking], [human_preferences])."""
+        import configparser
+        from .envs.env import CONFIG_INI
+        cfg = configparser.ConfigParser()
+        cfg.read_string(CONFIG_INI)
+        d, hp = cfg['drinking'], cfg['human_preferences']
+        P = capi.AgDrinkingParams()
+        P.robot_body, P.tool_body = self.robot, self.tool
+        P.human_body_m, P.human_body_f = self.humans['male'], self.humans['female']
+        for i, l in enumerate(self.arm_links):
+            P.arm_links[i], P.arm_lower[i], P.arm_upper[i] = l, self.arm_lower[i], self.arm_upper[i]
+        P.ee_link = self.ee_link
+        P.head_link_m, P.head_link_f = self.gl(self.humans['male'], HEAD_LINK), self.gl(self.humans['female'], HEAD_LINK)
+        P.water_body0, P.n_water = self.waters[0], len(self.waters)
+        if list(self.waters) != list(range(self.waters[0], self.waters[0] + len(self.waters))):
+            raise ValueError('the water particles must be consecutive bodies')
+        fp, fq = self.cup_frame(np.zeros((1, 3)), np.array([[0, 0, 0, 1.0]]))
+        for i in range(3):
+            P.mouth_m[i], P.mouth_f[i] = self.mouth['male'][i], self.mouth['female'][i]
+            P.cup_frame_pos[i] = fp[0, i]
+            P.cup_top[i], P.cup_bottom[i] = CUP_TOP_CENTER_OFFSET[i], CUP_BOTTOM_CENTER_OFFSET[i]
+        for i in range(4):
+            P.cup_frame_quat[i] = fq[0, i]
+        P.action_multiplier, P.frame_skip = 0.05, 5
+        P.w_distance, P.w_action = float(d['distance_weight']), float(d['action_weight'])
+        P.w_cup_tilt, P.w_drinking = float(d['cup_tilt_weight']), float(d['drinking_reward_weight'])
+        P.c_v, P.c_f, P.c_hf = float(hp['velocity_weight']), float(hp['force_nontarget_weight']), float(hp['high_forces_weight'])
+        P.c_fd, P.c_fdv = float(hp['food_hit_weight']), float(hp['food_velocities_weight'])
+        P.task_success_threshold = float(d['task_success_threshold'])
+        P.seed = seed
+        return P
+
+    def start_fused(self, sim, sample=None, seed=1001):
+        """Arm the fused step (`sim.drinking_step_*`) for the envs last put in place by `reset` (or `sample`): a new episode with
+        every particle in play.  Draws nothing from the reset's generator."""
+        s = sample or self.last_sample
+        sim.drinking_init(self.drinking_params(seed), s['male'])
 
     def cup_frame(self, cup_pos, cup_quat):
         """drinking.py:25-26: the cup's frame used for its top / bottom centres: shifted by (0, 0.06, 0) and turned by 90 degrees about x."""

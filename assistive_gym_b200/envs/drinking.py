@@ -1,7 +1,9 @@
-"""`DrinkingEnv` (reference envs/drinking.py) on the batched backend, per-call API path: `step` = `take_step` + `_get_obs` +
+"""`DrinkingEnv` (reference envs/drinking.py) on the batched backend.  `step` is the per-call API path: `take_step` + `_get_obs` +
 `get_water_rewards` + `human_preferences` through the `Agent` getters, vectorised over `n_envs` (the per-particle Python loops of
-drinking.py:51-82 become masks over [n_envs][64]).  No fused kernels yet; checked on the CPU against the reference's own step code
-(tests/test_reference_drinking_semantics.py), not run on a GPU in the round that added it."""
+drinking.py:51-82 become masks over [n_envs][64]), checked against the reference's own step code
+(tests/test_reference_drinking_semantics.py).  `step_fused` runs the same step on the fused device kernels (ag_drinking.cuh,
+`ag_drinking_step_host`), armed by `reset`, and returns exactly what `step` returns; `AssistiveVecEnv` steps those kernels with
+device tensors."""
 import numpy as np
 
 from ..drinking_batch import CUP_BOTTOM_CENTER_OFFSET, CUP_TOP_CENTER_OFFSET, N_WATER, DrinkingBatch
@@ -41,6 +43,7 @@ class DrinkingEnv(AssistiveEnv):
         rng = np.random.default_rng(self.np_random.randint(0, 2 ** 31 - 1))
         s = db.reset(self.id, rng, settle_steps=50, impairment='no_tremor')
         self.start_episode(s)
+        db.start_fused(self.id, s, seed=self._seed)
         return self._squeeze(self._get_obs())
 
     def attach(self, sim):
@@ -96,6 +99,25 @@ class DrinkingEnv(AssistiveEnv):
                   self.config('cup_tilt_weight') * reward_tilt + self.config('drinking_reward_weight') * reward_water + pref)
         done = np.full(self.n_envs, self.iteration >= 200)
         info = {'total_force_on_human': self.total_force_on_human, 'task_success': (self.task_success >= self.total_water_count * self.config('task_success_threshold')).astype(int),
+                'action_robot_len': self.action_robot_len, 'action_human_len': self.action_human_len, 'obs_robot_len': self.obs_robot_len, 'obs_human_len': self.obs_human_len}
+        if self.n_envs == 1:
+            return obs[0], float(reward[0]), bool(done[0]), {k_: (v[0] if isinstance(v, np.ndarray) else v) for k_, v in info.items()}
+        return obs, reward, done, info
+
+    def step_fused(self, action):
+        """`step` on the fused, graph-replayed device path (armed by `reset`): takes and returns exactly what `step` does, and
+        leaves `waters`, `waters_active` and `task_success` as `step` would."""
+        a = np.asarray(action, dtype=np.float32).reshape(self.n_envs, -1)
+        obs, rew, done, info = self.id.drinking_step_host(a)
+        self.iteration += 1
+        ts, w, wa = self.id.drinking_get_state()
+        bits = np.arange(N_WATER, dtype=np.uint64)
+        self.waters = ((w[:, None] >> bits) & np.uint64(1)).astype(bool)
+        self.waters_active = ((wa[:, None] >> bits) & np.uint64(1)).astype(bool)
+        self.task_success = ts.astype(int)
+        self.total_force_on_human, self.robot_force_on_human, self.cup_force_on_human = (info[:, k].astype(np.float64) for k in (0, 2, 3))
+        obs, reward, done = obs.astype(np.float64), rew.astype(np.float64), done > 0.5
+        info = {'total_force_on_human': self.total_force_on_human, 'task_success': info[:, 1].astype(int),
                 'action_robot_len': self.action_robot_len, 'action_human_len': self.action_human_len, 'obs_robot_len': self.obs_robot_len, 'obs_human_len': self.obs_human_len}
         if self.n_envs == 1:
             return obs[0], float(reward[0]), bool(done[0]), {k_: (v[0] if isinstance(v, np.ndarray) else v) for k_, v in info.items()}

@@ -29,7 +29,7 @@ def _i32(a):
 
 
 # floats per env of the robot's and the person's observation of each fused task, in AgCoopParams.task order
-_OBS_W = {'feeding': (25, 23), 'scratch': (30, 34), 'bathing': (24, 28), 'dressing': (24, 28)}
+_OBS_W = {'feeding': (25, 23), 'scratch': (30, 34), 'bathing': (24, 28), 'dressing': (24, 28), 'drinking': (25, 0)}
 _TASKS = tuple(_OBS_W)
 
 
@@ -370,6 +370,25 @@ class BatchSim:
 
     def dressing_step_dev(self, action_ptr, obs_ptr, reward_ptr, done_ptr, info_ptr):
         self._step_dev(self.lib.ag_dressing_step_dev, action_ptr, obs_ptr, reward_ptr, done_ptr, info_ptr)
+
+    # ---- fused drinking path
+    def drinking_init(self, params, gender_is_male):
+        self._drink_params = params
+        g = _i32(np.broadcast_to(np.asarray(gender_is_male, dtype=np.int32), (self.n,)))
+        self._ck(self.lib.ag_drinking_init(self.h, C.byref(params), _p(g)))
+
+    def drinking_step_host(self, action):
+        return self._step_host('drinking', action)
+
+    def drinking_step_dev(self, action_ptr, obs_ptr, reward_ptr, done_ptr, info_ptr):
+        self._step_dev(self.lib.ag_drinking_step_dev, action_ptr, obs_ptr, reward_ptr, done_ptr, info_ptr)
+
+    def drinking_get_state(self):
+        """(task_success int32 [n], waters uint64 [n], waters_active uint64 [n]): bit i of a mask is water particle i"""
+        ts = np.zeros(self.n, dtype=np.int32)
+        w, wa = np.zeros(self.n, dtype=np.uint64), np.zeros(self.n, dtype=np.uint64)
+        self._ck(self.lib.ag_drinking_get_state(self.h, _p(ts), _p(w), _p(wa)))
+        return ts, w, wa
 
     def feeding_reset_episode(self, mask=None):
         self._ck(self.lib.ag_feeding_reset_episode(self.h, _p(_i32(mask))))

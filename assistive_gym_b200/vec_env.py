@@ -2,7 +2,8 @@
 
 The reference trains one `gym.Env` per RLlib worker process (`learn.py:26,61-69`); here ONE object steps
 `n_envs` environments on one GPU.  `step(actions)` takes and returns torch CUDA tensors: the action tensor's
-`data_ptr()` goes straight into `ag_feeding_step_dev` / `ag_bathing_step_dev`, observations / rewards / dones are
+`data_ptr()` goes straight into the task's fused step (`ag_feeding_step_dev`, `ag_bathing_step_dev`, `ag_dressing_step_dev`,
+`ag_scratch_step_dev`, `ag_drinking_step_dev`), observations / rewards / dones are
 written into pre-allocated device tensors on the simulation's own stream, and nothing crosses PCIe.  Episodes of
 all envs have the same length (200 steps, feeding.py:37), so the batch resets together; `auto_reset` does it inside
 `step` the way vector-env wrappers do (the terminal observation is kept in `info['terminal_observation']`).
@@ -69,8 +70,10 @@ class AssistiveVecEnv:
         if self.coop:
             self._step_dev, self._step_host = sim.coop_step_dev, sim.coop_step_host
             return obs
-        self._step_dev = {'feeding': sim.feeding_step_dev, 'bed_bathing': sim.bathing_step_dev, 'dressing': sim.dressing_step_dev, 'scratch_itch': sim.scratch_step_dev}[self.task]
-        self._step_host = {'feeding': sim.feeding_step_host, 'bed_bathing': sim.bathing_step_host, 'dressing': sim.dressing_step_host, 'scratch_itch': sim.scratch_step_host}[self.task]
+        self._step_dev = {'feeding': sim.feeding_step_dev, 'bed_bathing': sim.bathing_step_dev, 'dressing': sim.dressing_step_dev, 'scratch_itch': sim.scratch_step_dev,
+                          'drinking': sim.drinking_step_dev}[self.task]
+        self._step_host = {'feeding': sim.feeding_step_host, 'bed_bathing': sim.bathing_step_host, 'dressing': sim.dressing_step_host, 'scratch_itch': sim.scratch_step_host,
+                           'drinking': sim.drinking_step_host}[self.task]
         return obs
 
     def _batch_obs(self, obs):

@@ -342,6 +342,36 @@ int ag_scratch_init(AgSim* sim, const AgScratchParams* p, const int32_t* gender_
 int ag_scratch_step_dev(AgSim* sim, const float* action_dev, float* obs_dev, float* reward_dev, float* done_dev, float* info_dev);
 int ag_scratch_step_host(AgSim* sim, const float* action, float* obs, float* reward, float* done, float* info);
 
+/* --- fused DrinkingEnv path (drinking.py:10-117 + env.py:174-274): action -> PD targets -> frame_skip x numSubSteps substeps ->
+ * obs [25] / reward / done, with the water bookkeeping of get_water_rewards (drinking.py:51-82): a particle outside the cup
+ * (util.points_in_cylinder, radius 0.05) within 0.03 m of the mouth is swallowed (+10, moved 1000-2000 m away), one outside the
+ * cup with no cup collider within 0.1 m is spilled (-1); particles that touch the person cost the food-hit preference. ------ */
+typedef struct AgDrinkingParams {
+  int32_t robot_body, tool_body, human_body_m, human_body_f;   /* tool_body: the cup */
+  int32_t arm_links[7];         /* controllable joints (global link ids) */
+  int32_t ee_link;              /* right_end_effector */
+  int32_t head_link_m, head_link_f;
+  int32_t water_body0, n_water; /* the water particles are bodies water_body0 .. water_body0 + n_water - 1 (n_water <= 64) */
+  float   arm_lower[7], arm_upper[7];
+  float   mouth_m[3], mouth_f[3];
+  float   cup_frame_pos[3], cup_frame_quat[4];  /* drinking.py:25-26: the frame of the cup's centres in its COM frame */
+  float   cup_top[3], cup_bottom[3];            /* the top / bottom centre in that frame (drinking.py:137-138) */
+  float   action_multiplier;    /* 0.05 env.py:188 */
+  int32_t frame_skip;           /* 5 */
+  float   w_distance, w_action, w_cup_tilt, w_drinking; /* config.ini [drinking] */
+  float   c_v, c_f, c_hf, c_fd, c_fdv;                  /* config.ini [human_preferences] */
+  float   task_success_threshold;
+  uint64_t seed;                /* of the per-env generator that places swallowed particles */
+} AgDrinkingParams;
+/* Allocates at the first call; every call re-arms the episode: iteration 0, no particle swallowed, all particles present. */
+int ag_drinking_init(AgSim* sim, const AgDrinkingParams* p, const int32_t* gender_is_male);
+/* obs [N][25], reward [N], done [N], info [N][4] = total force on the person, task success, robot force, cup force on the person */
+int ag_drinking_step_dev(AgSim* sim, const float* action_dev, float* obs_dev, float* reward_dev, float* done_dev, float* info_dev);
+int ag_drinking_step_host(AgSim* sim, const float* action, float* obs, float* reward, float* done, float* info);
+/* the particle bookkeeping (host buffers, each may be NULL): swallowed particles [N]; bit i of waters [N] = particle i is still
+ * in play (self.waters), of waters_active [N] = it can still hit the person (self.waters_active) */
+int ag_drinking_get_state(AgSim* sim, int32_t* task_success, uint64_t* waters, uint64_t* waters_active);
+
 /* --- fused co-optimisation step (FeedingJacoHuman-v1, ScratchItchJacoHuman-v1, BedBathingSawyerHuman-v1, DressingPR2Human-v1; env.py:174-235 with the person as a second
  * agent): the robot part is the task's own fused step; the person's part applies the human slice of the action to its
  * controllable joints (clip to [-1, 1], x 0.05, 5-fold accumulate inside its limits), and after every stepSimulation
@@ -353,7 +383,8 @@ typedef struct AgCoopParams {
   int32_t task;                 /* 0 = FeedingEnv (after ag_feeding_init), 1 = ScratchItchEnv (after ag_scratch_init),
                                    2 = BedBathingEnv (after ag_bathing_init and ag_bathing_set_target_frames),
                                    3 = DressingEnv (after ag_dressing_init; the left arm, with the gown stepped as in
-                                   ag_dressing_step: after every stepSimulation the limits, then the anchor follows) */
+                                   ag_dressing_step: after every stepSimulation the limits, then the anchor follows);
+                                   4 is reserved for DrinkingEnv and not built yet */
   int32_t human_body_m, human_body_f;
   int32_t n_joints;             /* every joint of the person: enforce_joint_limits clamps all of them */
   int32_t joint_links_m[AG_COOP_MAXJ], joint_links_f[AG_COOP_MAXJ];   /* global link ids per gender */
