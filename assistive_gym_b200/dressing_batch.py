@@ -30,7 +30,7 @@ from .feeding_batch import coop_params, pack_mlp
 from .human_model import create_human
 from .kinematics import BodyKinematics, q_axis, q_from_rpy, q_mul, q_rot
 from .toc import jlwki, position_robot_toc  # noqa: F401
-from .scene import JOINT_FIXED, JOINT_PRISMATIC, JOINT_REVOLUTE, SceneBuilder, quat_from_rpy, quat_mul, quat_rotate
+from .scene import SceneBuilder, quat_from_rpy
 
 MOTOR_POSITION = 1
 
@@ -101,22 +101,8 @@ class DressingBatch:
             b.set_gravity([0, 0, -1], body=hb)                                        # dressing.py:181
             self.humans[gender] = hb
         self.robot = b.load_urdf('pr2', base_pos=[-1, -1, 0], fixed_base=True, inertia_from_file=True)    # pr2.py:52
-        live = set(PR2['arm']) | set(PR2['gripper'])
-        preset = dict(zip(PR2['right_arm'], PR2['right_preset']))
-        for j in range(b.num_joints(self.robot)):
-            lk = b.links[b.global_link(self.robot, j)]
-            if j in live or lk.jtype == JOINT_FIXED:
-                continue
-            q0 = preset.get(j, 0.0)
-            if lk.jtype == JOINT_REVOLUTE:
-                lk.jquat = quat_mul(lk.jquat, np.array(list(np.asarray(lk.axis) * np.sin(q0 / 2)) + [np.cos(q0 / 2)]))
-            elif lk.jtype == JOINT_PRISMATIC:
-                lk.jpos = lk.jpos + quat_rotate(lk.jquat, lk.axis * q0)
-            lk.jtype, lk.haslimit = JOINT_FIXED, 0
-        for j in PR2['arm']:          # continuous joints without URDF limits: PyBullet reports (0, -1), the reference turns that
-            lk = b.links[b.global_link(self.robot, j)]     # into +-2 pi for IK and +-1e10 for the action clamp (agent.py:222-229)
-            if not lk.haslimit and lk.lower == lk.upper:
-                lk.lower, lk.upper = -2 * np.pi, 2 * np.pi
+        b.weld_joints(self.robot, set(PR2['arm']) | set(PR2['gripper']), dict(zip(PR2['right_arm'], PR2['right_preset'])))
+        b.continuous_limits_for_ik(self.robot, PR2['arm'])
         b.set_gravity([0, 0, 0], body=self.robot)                                     # dressing.py:179-180
         self.scene = b.finalize()
         sc = self.scene

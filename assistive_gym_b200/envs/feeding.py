@@ -16,14 +16,24 @@ from .agents.furniture import Furniture
 from .env import AssistiveEnv
 
 
+def feeding_batch_for(robot):
+    """The batched scene of `robot`'s Feeding id: the wheelchair-mounted Jaco, or Sawyer / PR2 placed by TOC."""
+    from ..feeding_robots_batch import FeedingPR2Batch, FeedingSawyerBatch
+    from .agents.robot import PR2, Jaco, Sawyer
+    for cls, batch in ((Jaco, FeedingBatch), (Sawyer, FeedingSawyerBatch), (PR2, FeedingPR2Batch)):
+        if type(robot) is cls:
+            return batch()
+    raise KeyError('Feeding is not built for %s' % type(robot).__name__)
+
+
 class FeedingEnv(AssistiveEnv):
     def __init__(self, robot, human, n_envs=1, device=0, seed=1001, config=None):
         super().__init__(robot=robot, human=human, task='feeding', n_envs=n_envs, device=device, seed=seed,
                          obs_robot_len=(18 + len(robot.controllable_joint_indices) - (len(robot.wheel_joint_indices) if robot.mobile else 0)),
                          obs_human_len=(19 + len(human.controllable_joint_indices)))
-        self._fb = FeedingBatch()
+        self._fb = feeding_batch_for(robot)
         self.human_impairment = 'random'      # build_assistive_env(human_impairment='random'), env.py:114
-        self._cfg = config or capi.default_config()
+        self._cfg = config or self._fb.config()
         self._sim_lib = None
         self.total_food_count = 8
 

@@ -1,5 +1,5 @@
 from .agents.human import Human, head_joints
-from .agents.robot import Jaco
+from .agents.robot import PR2, Jaco, Sawyer
 from .feeding import FeedingEnv
 
 robot_arm = 'right'
@@ -21,4 +21,36 @@ class FeedingJacoHumanEnv(FeedingEnv):
 
     def __init__(self, n_envs=1, device=0, seed=1001, config=None):
         super().__init__(robot=Jaco(robot_arm), human=Human(human_controllable_joint_indices, controllable=True),
+                         n_envs=n_envs, device=device, seed=seed, config=config)
+
+
+class FeedingSawyerEnv(FeedingEnv):
+    """`assistive_gym:FeedingSawyer-v1` (reference envs/feeding_envs.py:25-27): Sawyer beside the wheelchair, its base placed by TOC."""
+
+    def __init__(self, n_envs=1, device=0, seed=1001, config=None):
+        super().__init__(robot=Sawyer(robot_arm), human=Human(human_controllable_joint_indices, controllable=False),
+                         n_envs=n_envs, device=device, seed=seed, config=config)
+
+
+class FeedingPR2Env(FeedingEnv):
+    """`assistive_gym:FeedingPR2-v1` (reference envs/feeding_envs.py:17-19): PR2's right arm, its base placed by TOC."""
+
+    def __init__(self, n_envs=1, device=0, seed=1001, config=None):
+        super().__init__(robot=PR2(robot_arm), human=Human(human_controllable_joint_indices, controllable=False),
+                         n_envs=n_envs, device=device, seed=seed, config=config)
+
+
+class FeedingSawyerHumanEnv(FeedingEnv):
+    """`assistive_gym:FeedingSawyerHuman-v1` (reference envs/feeding_envs.py:51-54): as FeedingJacoHuman-v1, with Sawyer."""
+
+    def __init__(self, n_envs=1, device=0, seed=1001, config=None):
+        super().__init__(robot=Sawyer(robot_arm), human=Human(human_controllable_joint_indices, controllable=True),
+                         n_envs=n_envs, device=device, seed=seed, config=config)
+
+
+class FeedingPR2HumanEnv(FeedingEnv):
+    """`assistive_gym:FeedingPR2Human-v1` (reference envs/feeding_envs.py:41-44): as FeedingJacoHuman-v1, with PR2's right arm."""
+
+    def __init__(self, n_envs=1, device=0, seed=1001, config=None):
+        super().__init__(robot=PR2(robot_arm), human=Human(human_controllable_joint_indices, controllable=True),
                          n_envs=n_envs, device=device, seed=seed, config=config)

@@ -126,6 +126,11 @@ class FeedingBatch:
         self.hkin = {g: BodyKinematics(sc, hb) for g, hb in self.humans.items()}
         self.mouth = {'male': np.array([0, -0.11, 0.03]), 'female': np.array([0, -0.1, 0.03])}
 
+    @staticmethod
+    def config(**kw):
+        """AgConfig of the template: the default one."""
+        return capi.default_config(**kw)
+
     # ------------------------------------------------------------------ params for the fused kernels
     def feeding_params(self, seed=1001):
         P = capi.AgFeedingParams()
@@ -243,12 +248,20 @@ class FeedingBatch:
     def reset(self, sim, rng, settle_steps=25, sample=None, impairment='random', simulate_head=False):
         """Put every env of `sim` (BatchSim or the oracle wrapper) into a fresh FeedingJaco start state."""
         n = sim.n
-        sc = self.scene
         s = sample or self.sample(n, rng, impairment)
         self.last_sample = s
-        male = s['male'].astype(bool)
         if 'impairment' not in s:        # older fixtures: no impairment -> static humans
             s = dict(s, impairment=np.zeros(n, np.int32), tremors=np.zeros((n, 4)))
+        self._reset_person(sim, s, simulate_head)
+        sp = self._reset_wheelchair_robot(sim, s, rng)
+        self._reset_bowl_food(sim, s, sp, settle_steps)
+        return s
+
+    def _reset_person(self, sim, s, simulate_head):
+        """Ground friction and the seated person of the sampled gender: presets, random head angles, head motors (feeding.py:121-127)."""
+        n = sim.n
+        sc = self.scene
+        male = s['male'].astype(bool)
         tremor = s['impairment'] == 3
         sim.set_link_friction(int(sc['body_link0'][self.plane]), s['plane_friction'])
         # humans: presets + random head, only the sampled gender active
@@ -275,6 +288,11 @@ class FeedingBatch:
             sim.set_motor(hl, MOTOR_POSITION, target=rest, kp=[0.025] * 4, kd=[1.0] * 4, max_force=[1.0] * 4)
             sim.set_hard_limits(hl, True)
         self.human_q = q
+
+    def _reset_wheelchair_robot(self, sim, s, rng):
+        """The wheelchair-mounted arm's start pose (init_robot_pose's ik_random_restarts branch, env.py:293-296); returns the
+        spoon's placement."""
+        n = sim.n
         # robot: IK to the randomised end-effector target, gripper open
         target = np.array([-0.15, -0.65, 1.15]) + s['ee_offset']
         qik, ik_err = self.solve_ik(n, target, rng, sim=sim)
@@ -323,6 +341,12 @@ class FeedingBatch:
         zero3 = np.zeros((n, 3))
         sim.set_base_pose(self.tool, sp, sq)
         sim.set_base_velocity(self.tool, zero3, zero3)
+        return sp
+
+    def _reset_bowl_food(self, sim, s, sp, settle_steps):
+        """Bowl on the table, eight food particles above the spoon at `sp`, then the settle."""
+        n = sim.n
+        zero3 = np.zeros((n, 3))
         # bowl on the table
         sim.set_base_pose(self.bowl, np.array([-0.15, -0.65, 0.75]) + s['bowl_offset'], np.array([0, 0, 0, 1.0]))
         sim.set_base_velocity(self.bowl, zero3, zero3)
@@ -338,4 +362,3 @@ class FeedingBatch:
         sim.forward_kinematics()
         if settle_steps:
             sim.step(settle_steps)     # "drop food in the spoon" (feeding.py:178-179)
-        return s

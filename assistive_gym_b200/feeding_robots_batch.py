@@ -1,0 +1,191 @@
+"""FeedingSawyer-v1 and FeedingPR2-v1 (and their co-optimisation ids) as batched scenes: template construction and batched reset.
+
+The scene is FeedingJaco's -- person pair, wheelchair, table, bowl, the spoon on a fixed constraint, eight food spheres -- with another
+robot.  Robots that are not wheelchair-mounted load the plain wheelchair (furniture.py:16) and find their base pose with
+`init_robot_pose`'s TOC branch (env.py:276-310 -> robot.py:123-215): `attempts` random base poses beside the person, ranked by goals
+reached and JLWKI, then a collision check of robot and spoon against person, table and wheelchair, re-searching only the colliding
+envs for up to `max_iterations` rounds.  The goals are feeding.py:141's: two start goals (the randomised spoon pose with the task's
+end-effector orientation, and the mouth by position) that a base pose must both reach, and one target goal (the mouth with the
+end-effector orientation).  The task constants are the reference's `'feeding'` entries of agents/sawyer.py:8-47 and agents/pr2.py:8-47.
+
+Differences forced by the per-env DoF budget (32 per env, 16 per articulation; DESIGN.md section 9):
+  * Sawyer: the 7 arm joints and the 2 gripper joints are simulated; every other joint (the head pan) is welded at 0.
+  * PR2: the right arm (7) and the right gripper (4) are simulated; every other joint is welded at the angle `reset_joints` gives it
+    (pr2.py:60-66: the left arm at [1.75, 1.25, 1.5, -0.5, 1, 0, 1], all others 0), as dressing_batch.py does for the other arm.
+Neither robot is `mobile`, so gravity on it is off (feeding.py:150-151)."""
+import numpy as np
+
+from .feeding_batch import HEAD_LINK, TREMOR_JOINTS, FeedingBatch
+from .human_model import create_human
+from .kinematics import BodyKinematics, q_from_rpy, q_mul, q_rot
+from .scene import SceneBuilder, quat_from_rpy
+from .toc import position_robot_toc
+
+MOTOR_POSITION = 1
+
+SAWYER = dict(asset='sawyer', base_pos=[-1, -1, 0.975], load=dict(self_collision=True),
+              arm=[3, 8, 9, 10, 11, 13, 16], ee=19, gripper=[20, 22], tool_joint=18, gripper_collision=[18, 20, 21, 22, 23],
+              gripper_pos=[0.0, 0.0], tool_pos_offset=[-0.1, 0.12, -0.02], tool_orient_offset=[np.pi / 2.0 - 0.1, 0, np.pi / 2.0],
+              toc_base_pos_offset=[-0.1, 0.2, 0.975], ee_orient_rpy=[np.pi / 2.0, 0, np.pi / 2.0], weld_preset={}, default_q=None)
+PR2 = dict(asset='pr2', base_pos=[-1, -1, 0], load=dict(inertia_from_file=True),
+           arm=[42, 43, 44, 46, 47, 49, 50], ee=54, gripper=[57, 58, 59, 60], tool_joint=54, gripper_collision=list(range(49, 64)),
+           gripper_pos=[0.03] * 4, tool_pos_offset=[0, -0.03, -0.11], tool_orient_offset=[-0.2, 0, 0],
+           toc_base_pos_offset=[0.1, 0.2, 0], ee_orient_rpy=[np.pi / 2.0, 0, 0],
+           weld_preset=dict(zip([64, 65, 66, 68, 69, 71, 72], [1.75, 1.25, 1.5, -0.5, 1, 0, 1])),
+           default_q=[-1.75, 1.25, -1.5, -0.5, -1, 0, -1])
+TARGET_EE_POS = np.array([-0.15, -0.65, 1.15])       # feeding.py:139
+
+
+class FeedingTocBatch(FeedingBatch):
+    """Feeding with a robot placed by TOC.  Shares `sample`, the person, the bowl and the food, `feeding_params`, `start_fused` and
+    `start_coop` with `FeedingBatch`; FeedingJaco's own template and reset are not touched."""
+    R = None
+
+    def __init__(self):
+        R = self.R
+        b = SceneBuilder()
+        self.builder = b
+        b.set_gravity([0, 0, -9.81])
+        self.plane = b.load_urdf('plane')
+        self.robot = b.load_urdf(R['asset'], base_pos=R['base_pos'], fixed_base=True, **R['load'])
+        if R['asset'] == 'sawyer':                       # sawyer.py:55-61
+            for i in range(3, 24):
+                for j in range(3, 24):
+                    b.set_collision_filter_pair(self.robot, self.robot, i, j, False)
+            for i in range(0, 3):
+                for j in range(0, 9):
+                    b.set_collision_filter_pair(self.robot, self.robot, i, j, False)
+        b.weld_joints(self.robot, set(R['arm']) | set(R['gripper']), R['weld_preset'])
+        b.continuous_limits_for_ik(self.robot, R['arm'])
+        self.humans = {}
+        for gender, z in (('male', 0.89), ('female', 0.86)):
+            hb, info = create_human(b, gender=gender, static=True)
+            b.bodies[hb].base_pos = np.array([0, 0.03, z])
+            for j in range(b.num_joints(hb)):
+                if j not in TREMOR_JOINTS:
+                    b.change_dynamics(hb, j, mass=0)
+            self.humans[gender] = hb
+        self.wheelchair = b.load_urdf('wheelchair', base_pos=[0, 0, 0.06], fixed_base=False)     # furniture.py:16, not mounted
+        self.table = b.load_urdf('table_tall', base_pos=[0.25, -1.0, 0])
+        sp_shape = b.create_collision_shape('mesh', mesh_asset='spoon_vhacd', mesh_scale=[0.08] * 3)
+        self.tool = b.create_multibody(base_mass=1.0, base_shape=sp_shape, name='spoon')
+        for j in R['gripper_collision']:
+            b.set_collision_filter_pair(self.robot, self.tool, j, -1, False)
+        self.tool_pos_offset = np.array(R['tool_pos_offset'], dtype=np.float64)
+        self.tool_quat_offset = quat_from_rpy(R['tool_orient_offset'])
+        b.create_fixed_constraint(self.robot, R['tool_joint'], self.tool, -1, self.tool_pos_offset, [0, 0, 0],
+                                  self.tool_quat_offset, [0, 0, 0, 1], max_force=500)
+        self.bowl = b.load_urdf('bowl', base_pos=[-0.15, -0.65, 0.75])
+        fs = b.create_collision_shape('sphere', radius=0.005)
+        self.foods = [b.create_multibody(base_mass=0.001, base_shape=fs, name='food%d' % i) for i in range(8)]
+        b.set_gravity([0, 0, 0], body=self.robot)
+        for hb in self.humans.values():
+            b.set_gravity([0, 0, 0], body=hb)
+        b.set_gravity([0, 0, 0], body=self.tool)
+        self.scene = b.finalize()
+        sc = self.scene
+        self.gl = lambda body, link: int(sc['body_link0'][body]) + 1 + link
+        self.arm_links = [self.gl(self.robot, j) for j in R['arm']]
+        self.gripper_links = [self.gl(self.robot, j) for j in R['gripper']]
+        self.ee_link = self.gl(self.robot, R['ee'])
+        self.kin = BodyKinematics(sc, self.robot)
+        self.arm_lower = sc['link_lower'][self.arm_links].copy()
+        self.arm_upper = sc['link_upper'][self.arm_links].copy()
+        nolimit = sc['link_haslimit'][self.arm_links] == 0
+        self.arm_lower[nolimit], self.arm_upper[nolimit] = -1e10, 1e10
+        self.hkin = {g: BodyKinematics(sc, hb) for g, hb in self.humans.items()}
+        self.mouth = {'male': np.array([0, -0.11, 0.03]), 'female': np.array([0, -0.1, 0.03])}
+        self.robot_base_pos = np.array(R['base_pos'], dtype=np.float64)
+        self.robot_base_quat = np.array([0, 0, 0, 1.0])
+
+    def reset(self, sim, rng, settle_steps=25, sample=None, impairment='random', simulate_head=False, attempts=50, max_iterations=3):
+        """Put every env of `sim` into a fresh start state.  A sample that holds `base_pos`, `base_quat` and `q7` (as `reset` leaves
+        it) replays that robot placement instead of searching."""
+        n = sim.n
+        s = dict(sample) if sample else self.sample(n, rng, impairment)
+        self.last_sample = s
+        self._reset_person(sim, s, simulate_head)
+        sp = self._reset_toc_robot(sim, s, rng, attempts, max_iterations)
+        self._reset_bowl_food(sim, s, sp, settle_steps)
+        return s
+
+    def mouth_target(self, sim, male):
+        """generate_target (feeding.py:185-190): the mouth offset in the active person's head frame."""
+        sim.forward_kinematics()
+        out = np.zeros((sim.n, 3))
+        for g, hb in self.humans.items():
+            on = male if g == 'male' else ~male
+            st = sim.get_link_states([self.gl(hb, HEAD_LINK)])
+            hp, hq = st['pos'][:, 0].astype(np.float64), st['quat'][:, 0].astype(np.float64)
+            out[on] = (hp + q_rot(hq, np.broadcast_to(self.mouth[g], hp.shape)))[on]
+        return out
+
+    def place_robot(self, sim, base_pos, base_quat, q7):
+        """Robot base, arm, open gripper and the spoon at the tool joint's COM frame composed with the offsets (tool.py:49-54);
+        returns the spoon's position."""
+        n, R = sim.n, self.R
+        sim.set_base_pose(self.robot, base_pos, base_quat)
+        sim.set_base_velocity(self.robot, np.zeros((n, 3)), np.zeros((n, 3)))
+        sim.set_joint_state(self.arm_links, q=q7, qd=np.zeros_like(q7))
+        gq = np.tile(R['gripper_pos'], (n, 1)).astype(np.float64)
+        sim.set_joint_state(self.gripper_links, q=gq, qd=np.zeros_like(gq))
+        qfull = np.zeros((n, self.kin.nl))
+        qfull[:, np.array(R['arm']) + 1] = q7
+        qfull[:, np.array(R['gripper']) + 1] = gq
+        pos, quat = self.kin.fk(base_pos, base_quat, qfull)
+        cp, cq = self.kin.link_com_pose(pos, quat, R['tool_joint'] + 1)
+        sp = cp + q_rot(cq, self.tool_pos_offset)
+        sq = q_mul(cq, np.broadcast_to(self.tool_quat_offset, (n, 4)))
+        sim.set_base_pose(self.tool, sp, sq)
+        sim.set_base_velocity(self.tool, np.zeros((n, 3)), np.zeros((n, 3)))
+        sim.forward_kinematics()
+        return sp
+
+    def colliding(self, sim):
+        """env.py:300-309: robot or spoon touching the person, the table or the wheelchair."""
+        hit = np.zeros(sim.n, dtype=bool)
+        for ob in (self.humans['male'], self.humans['female'], self.table, self.wheelchair):
+            hit |= sim.closest_points(self.robot, ob, 0.0, max_pts=1)[1] > 0
+            hit |= sim.closest_points(self.tool, ob, 0.0, max_pts=1)[1] > 0
+        return hit
+
+    def _reset_toc_robot(self, sim, s, rng, attempts, max_iterations):
+        n, R = sim.n, self.R
+        male = s['male'].astype(bool)
+        if 'base_pos' in s:
+            base_pos, base_quat, q7 = s['base_pos'].copy(), s['base_quat'].copy(), s['q7'].copy()
+            self.goals_reached = s.get('goals_reached')
+            sp = self.place_robot(sim, base_pos, base_quat, q7)
+            self.unresolved = int(self.colliding(sim).sum())
+        else:
+            mouth = self.mouth_target(sim, male)
+            target = TARGET_EE_POS + s['ee_offset']
+            tq = np.tile(q_from_rpy(R['ee_orient_rpy']), (n, 1))
+            base0 = np.array([-0.85, -0.4, 0]) + np.array(R['toc_base_pos_offset'])
+            base_pos = np.zeros((n, 3)); base_quat = np.tile([0, 0, 0, 1.0], (n, 1)); q7 = np.zeros((n, 7)); reached = np.full(n, -1)
+            todo = np.ones(n, dtype=bool)
+            for _ in range(max_iterations):                                          # env.py:282
+                bp, bq, bj, num, _man = position_robot_toc(sim, rng, self.robot, self.arm_links, self.ee_link, self.kin, np.array(R['arm']) + 1,
+                                                           R['ee'] + 1, self.arm_lower, self.arm_upper, base0, [(target, tq), (mouth, None), (mouth, tq)],
+                                                           right_side=True, base_yaw=0.0, attempts=attempts, mask=todo, default_q=R['default_q'], n_start=2)
+                base_pos[todo], base_quat[todo], q7[todo], reached[todo] = bp[todo], bq[todo], bj[todo], num[todo]
+                sp = self.place_robot(sim, base_pos, base_quat, q7)
+                todo = self.colliding(sim)
+                if not todo.any():
+                    break
+            self.unresolved = int(todo.sum())
+            self.goals_reached = reached
+            s.update(base_pos=base_pos.copy(), base_quat=base_quat.copy(), q7=q7.copy(), goals_reached=reached.copy())
+        gq = np.tile(R['gripper_pos'], (n, 1)).astype(np.float64)
+        ng = len(R['gripper'])
+        sim.set_motor(self.arm_links, MOTOR_POSITION, target=q7, kp=[0.025] * 7, kd=[1.0] * 7, max_force=[1.0] * 7)       # feeding.py:122
+        sim.set_motor(self.gripper_links, MOTOR_POSITION, target=gq, kp=[0.05] * ng, kd=[1.0] * ng, max_force=[500.0] * ng)
+        return sp
+
+
+class FeedingSawyerBatch(FeedingTocBatch):
+    R = SAWYER
+
+
+class FeedingPR2Batch(FeedingTocBatch):
+    R = PR2

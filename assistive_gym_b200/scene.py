@@ -269,6 +269,27 @@ class SceneBuilder:
     def num_joints(self, body):
         return self.bodies[body].nlinks - 1
 
+    def weld_joints(self, body, live, preset):
+        """Turn every non-fixed joint of `body` outside `live` into a fixed one at its `preset` angle (a dict; default 0)."""
+        for j in range(self.num_joints(body)):
+            lk = self.links[self.global_link(body, j)]
+            if j in live or lk.jtype == JOINT_FIXED:
+                continue
+            q0 = preset.get(j, 0.0)
+            if lk.jtype == JOINT_REVOLUTE:
+                lk.jquat = quat_mul(lk.jquat, np.array(list(np.asarray(lk.axis) * np.sin(q0 / 2)) + [np.cos(q0 / 2)]))
+            elif lk.jtype == JOINT_PRISMATIC:
+                lk.jpos = lk.jpos + quat_rotate(lk.jquat, lk.axis * q0)
+            lk.jtype, lk.haslimit = JOINT_FIXED, 0
+
+    def continuous_limits_for_ik(self, body, joints):
+        """Continuous joints without URDF limits: PyBullet reports (0, -1), the reference turns that into +-2 pi for IK and +-1e10
+        for the action clamp (agent.py:222-229); the template keeps +-2 pi."""
+        for j in joints:
+            lk = self.links[self.global_link(body, j)]
+            if not lk.haslimit and lk.lower == lk.upper:
+                lk.lower, lk.upper = -2 * np.pi, 2 * np.pi
+
     # ----- loadURDF
     def load_urdf(self, asset, base_pos=(0, 0, 0), base_quat=(0, 0, 0, 1), fixed_base=False,
                   self_collision=False, inertia_from_file=False, global_scaling=1.0):

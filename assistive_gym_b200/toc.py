@@ -36,9 +36,10 @@ def arm_jacobian(kin, arm_local, ee_local, base_pos, base_quat, q):
 
 def position_robot_toc(sim, rng, robot_body, arm_links, ee_link, kin, arm_local, ee_local, lower, upper, base0, goals,
                        right_side=True, base_yaw=0.0, attempts=50, random_rotation=30.0, random_position=0.5, mask=None,
-                       default_q=None, extra_attempts=50):
-    """goals: [(target_pos [N,3], target_quat [N,4] or None)], the first one is the start goal.  Returns the best base
-    position / orientation, the start joint angles, goals reached (-1: no pose reaches the start goal) and the score."""
+                       default_q=None, extra_attempts=50, n_start=1):
+    """goals: [(target_pos [N,3], target_quat [N,4] or None)], the first `n_start` are the start goals (robot.py:191-195: a base pose
+    that misses any of them is discarded) and the start joint angles are the first one's.  Returns the best base position /
+    orientation, the start joint angles, goals reached (-1: no pose reaches the start goals) and the score."""
     n = sim.n
     mask = np.ones(n, dtype=bool) if mask is None else mask.copy()
     nj = len(arm_links)
@@ -68,6 +69,7 @@ def position_robot_toc(sim, rng, robot_body, arm_links, ee_link, kin, arm_local,
                 man += np.where(ok, score, 0.0)
             if j == 0:
                 q_start = q.astype(np.float64)
+            if j < n_start:
                 valid &= ok
         better = valid & (num > 0) & ((num > best_num) | ((num == best_num) & (man > best_man)))
         best_num[better], best_man[better] = num[better], man[better]
