@@ -2,13 +2,14 @@ from .bed_bathing_envs import BedBathingSawyerEnv, BedBathingSawyerHumanEnv  # n
 from .dressing_envs import DressingPR2Env, DressingPR2HumanEnv  # noqa: F401
 from .drinking_envs import DrinkingJacoEnv  # noqa: F401
 from .feeding_envs import FeedingJacoEnv, FeedingJacoHumanEnv, FeedingPR2Env, FeedingPR2HumanEnv, FeedingSawyerEnv, FeedingSawyerHumanEnv  # noqa: F401
-from .scratch_itch_envs import ScratchItchJacoEnv, ScratchItchJacoHumanEnv  # noqa: F401
+from .scratch_itch_envs import ScratchItchJacoEnv, ScratchItchJacoHumanEnv, ScratchItchPR2Env, ScratchItchPR2HumanEnv, ScratchItchSawyerEnv, ScratchItchSawyerHumanEnv  # noqa: F401
 
 ENV_REGISTRY = {'FeedingJaco-v1': FeedingJacoEnv, 'BedBathingSawyer-v1': BedBathingSawyerEnv, 'DressingPR2-v1': DressingPR2Env, 'ScratchItchJaco-v1': ScratchItchJacoEnv,
                 'FeedingJacoHuman-v1': FeedingJacoHumanEnv, 'ScratchItchJacoHuman-v1': ScratchItchJacoHumanEnv, 'DrinkingJaco-v1': DrinkingJacoEnv,
                 'BedBathingSawyerHuman-v1': BedBathingSawyerHumanEnv, 'DressingPR2Human-v1': DressingPR2HumanEnv,
                 'FeedingSawyer-v1': FeedingSawyerEnv, 'FeedingPR2-v1': FeedingPR2Env, 'FeedingSawyerHuman-v1': FeedingSawyerHumanEnv,
-                'FeedingPR2Human-v1': FeedingPR2HumanEnv}
+                'FeedingPR2Human-v1': FeedingPR2HumanEnv, 'ScratchItchSawyer-v1': ScratchItchSawyerEnv, 'ScratchItchPR2-v1': ScratchItchPR2Env,
+                'ScratchItchSawyerHuman-v1': ScratchItchSawyerHumanEnv, 'ScratchItchPR2Human-v1': ScratchItchPR2HumanEnv}
 
 
 def make(env_id, **kw):

@@ -1,6 +1,7 @@
 """`ScratchItchEnv` (reference envs/scratch_itch.py) on the batched backend: `step` runs the fused path
-(`ag_scratch_step_host`); `_get_obs` (used by `reset`) reads the same quantities through the per-call Agent API.
-With a controllable person (co-optimisation, `ScratchItchJacoHuman-v1`) `step` takes {'robot': a7, 'human': a10} and goes through
+(`ag_scratch_step_host`); `_get_obs` (used by `reset`) reads the same quantities through the per-call Agent API.  The robot is the
+wheelchair-mounted Jaco or Sawyer / PR2 placed by TOC (`scratch_itch_robots_batch.py`).
+With a controllable person (co-optimisation, `ScratchItchJacoHuman-v1`, `ScratchItchSawyerHuman-v1`, `ScratchItchPR2Human-v1`) `step` takes {'robot': a7, 'human': a10} and goes through
 the per-call path (`step_reference_api`): `take_step` drives the person's right arm too and keeps it inside the realistic joint
 limits (the MLP classifier of human.py:134-152) after every substep.  `step_fused` runs the same co-optimisation step on the
 device (`ag_coop_step_host`)."""
@@ -13,12 +14,22 @@ from ..sim import BatchSim
 from .env import AssistiveEnv
 
 
+def scratch_batch_for(robot):
+    """The batched scene of `robot`'s ScratchItch id: the wheelchair-mounted Jaco, or Sawyer / PR2 placed by TOC."""
+    from ..scratch_itch_robots_batch import ScratchItchPR2Batch, ScratchItchSawyerBatch
+    from .agents.robot import PR2, Jaco, Sawyer
+    for cls, batch in ((Jaco, ScratchItchBatch), (Sawyer, ScratchItchSawyerBatch), (PR2, ScratchItchPR2Batch)):
+        if type(robot) is cls:
+            return batch()
+    raise KeyError('ScratchItch is not built for %s' % type(robot).__name__)
+
+
 class ScratchItchEnv(AssistiveEnv):
     def __init__(self, robot, human, n_envs=1, device=0, seed=1001, config=None):
         super().__init__(robot=robot, human=human, task='scratch_itch', n_envs=n_envs, device=device, seed=seed,
                          obs_robot_len=(23 + len(robot.controllable_joint_indices) - (len(robot.wheel_joint_indices) if robot.mobile else 0)),
                          obs_human_len=(24 + len(human.controllable_joint_indices)))
-        self._sb = ScratchItchBatch()
+        self._sb = scratch_batch_for(robot)
         self._cfg = config or capi.default_config()
         self._sim_lib = None
 
@@ -92,7 +103,7 @@ class ScratchItchEnv(AssistiveEnv):
         total = sum(self.id.contact_force_sum(self.robot.body, h.body) for h in self.humans.values()).astype(np.float64)
         tool_force = self.id.contact_force_sum(self.tool.body).astype(np.float64)
         at_target, cpos = np.zeros(n), np.full((n, 3), np.nan)
-        tool_links = [self.tool.link0, self.tool.link0 + 1]                # linkA in [0, 1]: the handle and the tip
+        tool_links = [self.tool._gl(0), self.tool._gl(1)]                  # linkA in [0, 1]: the scratcher's links 0 and 1 (not its base)
         for h in self.humans.values():
             c, k = self.id.get_contacts(self.tool.body, h.body, max_pts=32)
             for i in range(int(k.max()) if n else 0):

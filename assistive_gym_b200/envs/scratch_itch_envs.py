@@ -1,5 +1,5 @@
 from .agents.human import Human, right_arm_joints
-from .agents.robot import Jaco
+from .agents.robot import PR2, Jaco, Sawyer
 from .scratch_itch import ScratchItchEnv
 
 robot_arm = 'left'
@@ -21,4 +21,36 @@ class ScratchItchJacoHumanEnv(ScratchItchEnv):
 
     def __init__(self, n_envs=1, device=0, seed=1001, config=None):
         super().__init__(robot=Jaco(robot_arm), human=Human(human_controllable_joint_indices, controllable=True),
+                         n_envs=n_envs, device=device, seed=seed, config=config)
+
+
+class ScratchItchSawyerEnv(ScratchItchEnv):
+    """`assistive_gym:ScratchItchSawyer-v1` (reference envs/scratch_itch_envs.py:25-27): Sawyer beside the wheelchair, its base placed by TOC."""
+
+    def __init__(self, n_envs=1, device=0, seed=1001, config=None):
+        super().__init__(robot=Sawyer(robot_arm), human=Human(human_controllable_joint_indices, controllable=False),
+                         n_envs=n_envs, device=device, seed=seed, config=config)
+
+
+class ScratchItchPR2Env(ScratchItchEnv):
+    """`assistive_gym:ScratchItchPR2-v1` (reference envs/scratch_itch_envs.py:17-19): PR2's left arm, its base placed by TOC."""
+
+    def __init__(self, n_envs=1, device=0, seed=1001, config=None):
+        super().__init__(robot=PR2(robot_arm), human=Human(human_controllable_joint_indices, controllable=False),
+                         n_envs=n_envs, device=device, seed=seed, config=config)
+
+
+class ScratchItchSawyerHumanEnv(ScratchItchEnv):
+    """`assistive_gym:ScratchItchSawyerHuman-v1` (reference envs/scratch_itch_envs.py:51-54): as ScratchItchJacoHuman-v1, with Sawyer."""
+
+    def __init__(self, n_envs=1, device=0, seed=1001, config=None):
+        super().__init__(robot=Sawyer(robot_arm), human=Human(human_controllable_joint_indices, controllable=True),
+                         n_envs=n_envs, device=device, seed=seed, config=config)
+
+
+class ScratchItchPR2HumanEnv(ScratchItchEnv):
+    """`assistive_gym:ScratchItchPR2Human-v1` (reference envs/scratch_itch_envs.py:41-44): as ScratchItchJacoHuman-v1, with PR2's left arm."""
+
+    def __init__(self, n_envs=1, device=0, seed=1001, config=None):
+        super().__init__(robot=PR2(robot_arm), human=Human(human_controllable_joint_indices, controllable=True),
                          n_envs=n_envs, device=device, seed=seed, config=config)

@@ -17,9 +17,9 @@ import numpy as np
 
 from .feeding_batch import HEAD_LINK, TREMOR_JOINTS, FeedingBatch
 from .human_model import create_human
-from .kinematics import BodyKinematics, q_from_rpy, q_mul, q_rot
+from .kinematics import BodyKinematics, q_from_rpy, q_rot
 from .scene import SceneBuilder, quat_from_rpy
-from .toc import position_robot_toc
+from .toc import TocPlacement
 
 MOTOR_POSITION = 1
 
@@ -36,7 +36,7 @@ PR2 = dict(asset='pr2', base_pos=[-1, -1, 0], load=dict(inertia_from_file=True),
 TARGET_EE_POS = np.array([-0.15, -0.65, 1.15])       # feeding.py:139
 
 
-class FeedingTocBatch(FeedingBatch):
+class FeedingTocBatch(TocPlacement, FeedingBatch):
     """Feeding with a robot placed by TOC.  Shares `sample`, the person, the bowl and the food, `feeding_params`, `start_fused` and
     `start_coop` with `FeedingBatch`; FeedingJaco's own template and reset are not touched."""
     R = None
@@ -97,6 +97,7 @@ class FeedingTocBatch(FeedingBatch):
         self.mouth = {'male': np.array([0, -0.11, 0.03]), 'female': np.array([0, -0.1, 0.03])}
         self.robot_base_pos = np.array(R['base_pos'], dtype=np.float64)
         self.robot_base_quat = np.array([0, 0, 0, 1.0])
+        self.obstacles = (self.humans['male'], self.humans['female'], self.table, self.wheelchair)     # env.py:300-309
 
     def reset(self, sim, rng, settle_steps=25, sample=None, impairment='random', simulate_head=False, attempts=50, max_iterations=3):
         """Put every env of `sim` into a fresh start state.  A sample that holds `base_pos`, `base_quat` and `q7` (as `reset` leaves
@@ -120,35 +121,6 @@ class FeedingTocBatch(FeedingBatch):
             out[on] = (hp + q_rot(hq, np.broadcast_to(self.mouth[g], hp.shape)))[on]
         return out
 
-    def place_robot(self, sim, base_pos, base_quat, q7):
-        """Robot base, arm, open gripper and the spoon at the tool joint's COM frame composed with the offsets (tool.py:49-54);
-        returns the spoon's position."""
-        n, R = sim.n, self.R
-        sim.set_base_pose(self.robot, base_pos, base_quat)
-        sim.set_base_velocity(self.robot, np.zeros((n, 3)), np.zeros((n, 3)))
-        sim.set_joint_state(self.arm_links, q=q7, qd=np.zeros_like(q7))
-        gq = np.tile(R['gripper_pos'], (n, 1)).astype(np.float64)
-        sim.set_joint_state(self.gripper_links, q=gq, qd=np.zeros_like(gq))
-        qfull = np.zeros((n, self.kin.nl))
-        qfull[:, np.array(R['arm']) + 1] = q7
-        qfull[:, np.array(R['gripper']) + 1] = gq
-        pos, quat = self.kin.fk(base_pos, base_quat, qfull)
-        cp, cq = self.kin.link_com_pose(pos, quat, R['tool_joint'] + 1)
-        sp = cp + q_rot(cq, self.tool_pos_offset)
-        sq = q_mul(cq, np.broadcast_to(self.tool_quat_offset, (n, 4)))
-        sim.set_base_pose(self.tool, sp, sq)
-        sim.set_base_velocity(self.tool, np.zeros((n, 3)), np.zeros((n, 3)))
-        sim.forward_kinematics()
-        return sp
-
-    def colliding(self, sim):
-        """env.py:300-309: robot or spoon touching the person, the table or the wheelchair."""
-        hit = np.zeros(sim.n, dtype=bool)
-        for ob in (self.humans['male'], self.humans['female'], self.table, self.wheelchair):
-            hit |= sim.closest_points(self.robot, ob, 0.0, max_pts=1)[1] > 0
-            hit |= sim.closest_points(self.tool, ob, 0.0, max_pts=1)[1] > 0
-        return hit
-
     def _reset_toc_robot(self, sim, s, rng, attempts, max_iterations):
         n, R = sim.n, self.R
         male = s['male'].astype(bool)
@@ -161,20 +133,8 @@ class FeedingTocBatch(FeedingBatch):
             mouth = self.mouth_target(sim, male)
             target = TARGET_EE_POS + s['ee_offset']
             tq = np.tile(q_from_rpy(R['ee_orient_rpy']), (n, 1))
-            base0 = np.array([-0.85, -0.4, 0]) + np.array(R['toc_base_pos_offset'])
-            base_pos = np.zeros((n, 3)); base_quat = np.tile([0, 0, 0, 1.0], (n, 1)); q7 = np.zeros((n, 7)); reached = np.full(n, -1)
-            todo = np.ones(n, dtype=bool)
-            for _ in range(max_iterations):                                          # env.py:282
-                bp, bq, bj, num, _man = position_robot_toc(sim, rng, self.robot, self.arm_links, self.ee_link, self.kin, np.array(R['arm']) + 1,
-                                                           R['ee'] + 1, self.arm_lower, self.arm_upper, base0, [(target, tq), (mouth, None), (mouth, tq)],
-                                                           right_side=True, base_yaw=0.0, attempts=attempts, mask=todo, default_q=R['default_q'], n_start=2)
-                base_pos[todo], base_quat[todo], q7[todo], reached[todo] = bp[todo], bq[todo], bj[todo], num[todo]
-                sp = self.place_robot(sim, base_pos, base_quat, q7)
-                todo = self.colliding(sim)
-                if not todo.any():
-                    break
-            self.unresolved = int(todo.sum())
-            self.goals_reached = reached
+            base_pos, base_quat, q7, sp = self.toc_search(sim, rng, [(target, tq), (mouth, None), (mouth, tq)], 2, attempts, max_iterations)
+            reached = self.goals_reached
             s.update(base_pos=base_pos.copy(), base_quat=base_quat.copy(), q7=q7.copy(), goals_reached=reached.copy())
         gq = np.tile(R['gripper_pos'], (n, 1)).astype(np.float64)
         ng = len(R['gripper'])

@@ -116,9 +116,16 @@ class ScratchItchBatch:
 
     def reset(self, sim, rng, sample=None):
         n = sim.n
-        sc = self.scene
         s = sample or self.sample(n, rng)
         self.last_sample = s
+        self._reset_person(sim, s)
+        self._reset_mounted_arm(sim, s, rng)
+        return s
+
+    def _reset_person(self, sim, s):
+        """Floor friction, both genders at ScratchItch's preset pose (one active per env), the right arm held by weak motors."""
+        n = sim.n
+        sc = self.scene
         male = s['male'].astype(bool)
         sim.set_link_friction(int(sc['body_link0'][self.plane]), s['plane_friction'])
         for g, hb in self.humans.items():
@@ -134,6 +141,9 @@ class ScratchItchBatch:
             al = self.human_arm_links[g]
             sim.set_motor(al, MOTOR_POSITION, target=np.tile(q[RIGHT_ARM_JOINTS], (n, 1)), kp=[0.01] * 10, kd=[1.0] * 10, max_force=[1.0] * 10)   # human.py:124-127
             sim.set_motor_force_scale(al, np.repeat(s['strength'][:, None], 10, axis=1))
+
+    def _reset_mounted_arm(self, sim, s, rng):
+        n = sim.n
         # robot: IK to the randomised end-effector pose, resampled while arm or tool touch the person / wheelchair (env.py:296-309)
         target = np.array([-0.6, 0, 0.8]) + s['ee_offset']
         tq = q_from_rpy(JACO['ee_orient_rpy'])
@@ -169,7 +179,6 @@ class ScratchItchBatch:
         sim.set_motor(self.arm_links, MOTOR_POSITION, target=q7, kp=[0.05] * 7, kd=[1.0] * 7, max_force=[1.0] * 7)          # robot.py:36-37
         sim.set_motor(self.gripper_links, MOTOR_POSITION, target=gq, kp=[0.05] * 3, kd=[1.0] * 3, max_force=[500.0] * 3)
         sim.forward_kinematics()
-        return s
 
     def limb_links(self, s):
         male = s['male'].astype(bool)

@@ -6,7 +6,7 @@ number of goals reached, ties by the sum over reached goals of the joint-limited
 arm Jacobian at the IK solution; a pose whose start goal is unreachable is discarded."""
 import numpy as np
 
-from .kinematics import q_rot
+from .kinematics import q_mul, q_rot
 
 
 def joint_limited_weighting(q, lower, upper):                    # robot.py:223-235
@@ -75,3 +75,59 @@ def position_robot_toc(sim, rng, robot_body, arm_links, ee_link, kin, arm_local,
         best_num[better], best_man[better] = num[better], man[better]
         best_pos[better], best_quat[better], best_q[better] = bp[better], bq[better], q_start[better]
     return best_pos, best_quat, best_q, best_num, best_man
+
+
+class TocPlacement:
+    """`init_robot_pose`'s TOC branch (env.py:276-310) for a batched scene whose robot is not wheelchair-mounted: a TOC search,
+    then a collision check of robot and tool against `obstacles`, re-searching only the colliding envs for up to `max_iterations`
+    rounds.  The scene class provides `R` (the robot's task constants), `robot`, `tool`, `kin`, `arm_links`, `gripper_links`,
+    `ee_link`, `arm_lower`, `arm_upper`, `tool_pos_offset`, `tool_quat_offset` and `obstacles`."""
+
+    def place_robot(self, sim, base_pos, base_quat, q7):
+        """Robot base, arm, open gripper and the tool at the tool joint's COM frame composed with the offsets (tool.py:49-54);
+        returns the tool's position."""
+        n, R = sim.n, self.R
+        sim.set_base_pose(self.robot, base_pos, base_quat)
+        sim.set_base_velocity(self.robot, np.zeros((n, 3)), np.zeros((n, 3)))
+        sim.set_joint_state(self.arm_links, q=q7, qd=np.zeros_like(q7))
+        gq = np.tile(R['gripper_pos'], (n, 1)).astype(np.float64)
+        sim.set_joint_state(self.gripper_links, q=gq, qd=np.zeros_like(gq))
+        qfull = np.zeros((n, self.kin.nl))
+        qfull[:, np.array(R['arm']) + 1] = q7
+        qfull[:, np.array(R['gripper']) + 1] = gq
+        pos, quat = self.kin.fk(base_pos, base_quat, qfull)
+        cp, cq = self.kin.link_com_pose(pos, quat, R['tool_joint'] + 1)
+        sp = cp + q_rot(cq, self.tool_pos_offset)
+        sq = q_mul(cq, np.broadcast_to(self.tool_quat_offset, (n, 4)))
+        sim.set_base_pose(self.tool, sp, sq)
+        sim.set_base_velocity(self.tool, np.zeros((n, 3)), np.zeros((n, 3)))
+        sim.forward_kinematics()
+        return sp
+
+    def colliding(self, sim):
+        """env.py:300-309: robot or tool touching one of the `obstacles`."""
+        hit = np.zeros(sim.n, dtype=bool)
+        for ob in self.obstacles:
+            hit |= sim.closest_points(self.robot, ob, 0.0, max_pts=1)[1] > 0
+            hit |= sim.closest_points(self.tool, ob, 0.0, max_pts=1)[1] > 0
+        return hit
+
+    def toc_search(self, sim, rng, goals, n_start, attempts, max_iterations):
+        """Search, place and check; sets `goals_reached` and `unresolved` (envs still colliding after the last round) and returns
+        base position, base orientation, start joint angles and the tool's position."""
+        n, R = sim.n, self.R
+        base0 = np.array([-0.85, -0.4, 0]) + np.array(R['toc_base_pos_offset'])
+        base_pos = np.zeros((n, 3)); base_quat = np.tile([0, 0, 0, 1.0], (n, 1)); q7 = np.zeros((n, 7)); reached = np.full(n, -1)
+        todo = np.ones(n, dtype=bool)
+        for _ in range(max_iterations):                                          # env.py:282
+            bp, bq, bj, num, _man = position_robot_toc(sim, rng, self.robot, self.arm_links, self.ee_link, self.kin, np.array(R['arm']) + 1,
+                                                       R['ee'] + 1, self.arm_lower, self.arm_upper, base0, goals, right_side=True, base_yaw=0.0,
+                                                       attempts=attempts, mask=todo, default_q=R['default_q'], n_start=n_start)
+            base_pos[todo], base_quat[todo], q7[todo], reached[todo] = bp[todo], bq[todo], bj[todo], num[todo]
+            sp = self.place_robot(sim, base_pos, base_quat, q7)
+            todo = self.colliding(sim)
+            if not todo.any():
+                break
+        self.unresolved = int(todo.sum())
+        self.goals_reached = reached
+        return base_pos, base_quat, q7, sp
