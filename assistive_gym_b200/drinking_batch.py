@@ -124,9 +124,18 @@ class DrinkingBatch(FeedingBatch):
 
     def reset(self, sim, rng, settle_steps=50, sample=None, impairment='random', simulate_head=False):
         n = sim.n
-        sc = self.scene
         s = sample or self.sample(n, rng, impairment)
         self.last_sample = s
+        self._reset_person(sim, s, simulate_head)
+        self._reset_mounted_arm(sim, s, rng)
+        self._reset_water(sim, settle_steps)
+        return s
+
+    def _reset_person(self, sim, s, simulate_head):
+        """Floor friction, both genders at Feeding's presets with the sampled head pose (one active per env), the head joints held by
+        weak motors."""
+        n = sim.n
+        sc = self.scene
         male = s['male'].astype(bool)
         tremor = s['impairment'] == 3
         sim.set_link_friction(int(sc['body_link0'][self.plane]), s['plane_friction'])
@@ -145,6 +154,9 @@ class DrinkingBatch(FeedingBatch):
             hl = [self.gl(hb, j) for j in TREMOR_JOINTS]
             sim.set_motor(hl, MOTOR_POSITION, target=q[:, list(TREMOR_JOINTS)], kp=[0.005] * 4, kd=[1.0] * 4, max_force=[1.0] * 4)     # drinking.py:126
             sim.set_hard_limits(hl, True)
+
+    def _reset_mounted_arm(self, sim, s, rng):
+        n = sim.n
         gq0 = np.full((n, 3), JACO['gripper_pos'])
         sim.set_joint_state(self.gripper_links, q=gq0, qd=np.zeros_like(gq0))
         if 'q7' in s:
@@ -176,7 +188,12 @@ class DrinkingBatch(FeedingBatch):
         sim.set_joint_state(self.arm_links, q=arm_q, qd=np.zeros_like(arm_q))
         sim.set_motor(self.arm_links, MOTOR_POSITION, target=arm_q, kp=[0.005] * 7, kd=[1.0] * 7, max_force=[1.0] * 7)              # drinking.py:126
         sim.set_motor(self.gripper_links, MOTOR_POSITION, target=gq, kp=[0.05] * 3, kd=[1.0] * 3, max_force=[500.0] * 3)
-        sp, sq = self._place_cup(sim, arm_q)
+        self._place_cup(sim, arm_q)
+
+    def _reset_water(self, sim, settle_steps):
+        """The 4 x 4 x 4 water grid over the cup's centre of mass, then the settle."""
+        n = sim.n
+        sc = self.scene
         zero3 = np.zeros((n, 3))
         # water above the cup (drinking.py:159-168): the cup's base position is its centre of mass frame, as PyBullet reports it
         sim.forward_kinematics()
@@ -192,7 +209,6 @@ class DrinkingBatch(FeedingBatch):
         sim.forward_kinematics()
         if settle_steps:
             sim.step(settle_steps)                                              # "drop water in the cup" (drinking.py:175-176)
-        return s
 
     def _place_cup(self, sim, arm_q):
         """the cup at the tool joint's COM frame composed with the offsets (tool.py:49-54)"""

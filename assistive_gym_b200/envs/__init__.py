@@ -1,6 +1,6 @@
 from .bed_bathing_envs import BedBathingSawyerEnv, BedBathingSawyerHumanEnv  # noqa: F401
 from .dressing_envs import DressingPR2Env, DressingPR2HumanEnv  # noqa: F401
-from .drinking_envs import DrinkingJacoEnv  # noqa: F401
+from .drinking_envs import DrinkingJacoEnv, DrinkingPR2Env, DrinkingSawyerEnv  # noqa: F401
 from .feeding_envs import FeedingJacoEnv, FeedingJacoHumanEnv, FeedingPR2Env, FeedingPR2HumanEnv, FeedingSawyerEnv, FeedingSawyerHumanEnv  # noqa: F401
 from .scratch_itch_envs import ScratchItchJacoEnv, ScratchItchJacoHumanEnv, ScratchItchPR2Env, ScratchItchPR2HumanEnv, ScratchItchSawyerEnv, ScratchItchSawyerHumanEnv  # noqa: F401
 
@@ -9,7 +9,8 @@ ENV_REGISTRY = {'FeedingJaco-v1': FeedingJacoEnv, 'BedBathingSawyer-v1': BedBath
                 'BedBathingSawyerHuman-v1': BedBathingSawyerHumanEnv, 'DressingPR2Human-v1': DressingPR2HumanEnv,
                 'FeedingSawyer-v1': FeedingSawyerEnv, 'FeedingPR2-v1': FeedingPR2Env, 'FeedingSawyerHuman-v1': FeedingSawyerHumanEnv,
                 'FeedingPR2Human-v1': FeedingPR2HumanEnv, 'ScratchItchSawyer-v1': ScratchItchSawyerEnv, 'ScratchItchPR2-v1': ScratchItchPR2Env,
-                'ScratchItchSawyerHuman-v1': ScratchItchSawyerHumanEnv, 'ScratchItchPR2Human-v1': ScratchItchPR2HumanEnv}
+                'ScratchItchSawyerHuman-v1': ScratchItchSawyerHumanEnv, 'ScratchItchPR2Human-v1': ScratchItchPR2HumanEnv,
+                'DrinkingSawyer-v1': DrinkingSawyerEnv, 'DrinkingPR2-v1': DrinkingPR2Env}
 
 
 def make(env_id, **kw):

@@ -91,13 +91,16 @@ class Sawyer(Robot):
 
 
 class PR2(Robot):
-    """reference envs/agents/pr2.py:7-49 (the constants of the ScratchItch, Feeding and Dressing hot paths; the wheel / right-arm
-    tables are kept because `controllable_joints` selects among them)."""
+    """reference envs/agents/pr2.py:7-49 (the constants of the ScratchItch, Feeding, Drinking and Dressing hot paths; the wheel /
+    right-arm tables are kept because `controllable_joints` selects among them)."""
 
     def __init__(self, controllable_joints='right'):
         super().__init__(controllable_joints, [42, 43, 44, 46, 47, 49, 50], [64, 65, 66, 68, 69, 71, 72], list(range(3, 15)), 54, 76,
-                         [57, 58, 59, 60], [79, 80, 81, 82], {'scratch_itch': [0.25] * 4, 'feeding': [0.03] * 4, 'dressing': [0] * 4}, 54, 76,
-                         {'scratch_itch': [0, 0, 0], 'feeding': [0, -0.03, -0.11]}, {'scratch_itch': [0, 0, 0], 'feeding': [-0.2, 0, 0]},
-                         list(range(49, 64)), list(range(71, 86)), {'scratch_itch': [0.1, 0, 0], 'feeding': [0.1, 0.2, 0], 'dressing': [1.7, 0.7, 0]},
-                         {'scratch_itch': [0, 0, 0], 'feeding': [np.pi / 2.0, 0, 0], 'dressing': [[0, 0, np.pi], [0, 0, np.pi * 3 / 2.0]]},
+                         [57, 58, 59, 60], [79, 80, 81, 82],
+                         {'scratch_itch': [0.25] * 4, 'feeding': [0.03] * 4, 'drinking': [0.45] * 4, 'dressing': [0] * 4}, 54, 76,
+                         {'scratch_itch': [0, 0, 0], 'feeding': [0, -0.03, -0.11], 'drinking': [-0.01, 0, -0.05]},
+                         {'scratch_itch': [0, 0, 0], 'feeding': [-0.2, 0, 0], 'drinking': [np.pi / 2.0, 0, 0]},
+                         list(range(49, 64)), list(range(71, 86)),
+                         {'scratch_itch': [0.1, 0, 0], 'feeding': [0.1, 0.2, 0], 'drinking': [0.2, 0.2, 0], 'dressing': [1.7, 0.7, 0]},
+                         {'scratch_itch': [0, 0, 0], 'feeding': [np.pi / 2.0, 0, 0], 'drinking': [0, 0, 0], 'dressing': [[0, 0, np.pi], [0, 0, np.pi * 3 / 2.0]]},
                          wheelchair_mounted=False, half_range=False)

@@ -3,7 +3,7 @@
 drinking.py:51-82 become masks over [n_envs][64]), checked against the reference's own step code
 (tests/test_reference_drinking_semantics.py).  `step_fused` runs the same step on the fused device kernels (ag_drinking.cuh,
 `ag_drinking_step_host`), armed by `reset`, and returns exactly what `step` returns; `AssistiveVecEnv` steps those kernels with
-device tensors."""
+device tensors.  The robot is the wheelchair-mounted Jaco or Sawyer / PR2 placed by TOC (`drinking_robots_batch.py`)."""
 import numpy as np
 
 from ..drinking_batch import CUP_BOTTOM_CENTER_OFFSET, CUP_TOP_CENTER_OFFSET, N_WATER, DrinkingBatch
@@ -22,12 +22,22 @@ def points_in_cylinder(pt1, pt2, r, q):
     return (np.einsum('nmk,nk->nm', a, vec) >= 0) & (np.einsum('nmk,nk->nm', b, vec) <= 0) & (np.linalg.norm(np.cross(a, vec[:, None, :]), axis=-1) <= const[:, None])
 
 
+def drinking_batch_for(robot):
+    """The batched scene of `robot`'s Drinking id: the wheelchair-mounted Jaco, or Sawyer / PR2 placed by TOC."""
+    from ..drinking_robots_batch import DrinkingPR2Batch, DrinkingSawyerBatch
+    from .agents.robot import PR2, Jaco, Sawyer
+    for cls, batch in ((Jaco, DrinkingBatch), (Sawyer, DrinkingSawyerBatch), (PR2, DrinkingPR2Batch)):
+        if type(robot) is cls:
+            return batch()
+    raise KeyError('Drinking is not built for %s' % type(robot).__name__)
+
+
 class DrinkingEnv(AssistiveEnv):
     def __init__(self, robot, human, n_envs=1, device=0, seed=1001, config=None):
         super().__init__(robot=robot, human=human, task='drinking', n_envs=n_envs, device=device, seed=seed,
                          obs_robot_len=(18 + len(robot.controllable_joint_indices) - (len(robot.wheel_joint_indices) if robot.mobile else 0)),
                          obs_human_len=(19 + len(human.controllable_joint_indices)))
-        self._db = DrinkingBatch()
+        self._db = drinking_batch_for(robot)
         self.human_impairment = 'random'
         self._cfg = config or DrinkingBatch.config()
         self._sim_lib = None

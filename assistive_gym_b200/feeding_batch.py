@@ -183,6 +183,17 @@ class FeedingBatch:
             rest[sel] = np.clip(rest[sel], self.scene['link_lower'][hl], self.scene['link_upper'][hl])
         return rest
 
+    def mouth_target(self, sim, male):
+        """generate_target (feeding.py:185-190): the mouth offset in the active person's head frame."""
+        sim.forward_kinematics()
+        out = np.zeros((sim.n, 3))
+        for g, hb in self.humans.items():
+            on = male if g == 'male' else ~male
+            st = sim.get_link_states([self.gl(hb, HEAD_LINK)])
+            hp, hq = st['pos'][:, 0].astype(np.float64), st['quat'][:, 0].astype(np.float64)
+            out[on] = (hp + q_rot(hq, np.broadcast_to(self.mouth[g], hp.shape)))[on]
+        return out
+
     # ------------------------------------------------------------------ batched reset
     def sample(self, n, rng, impairment='random'):
         """Per-env randomisation (env.py:120, human.py:76-92, feeding.py:125,139, furniture.py:33).

@@ -15,24 +15,19 @@ Differences forced by the per-env DoF budget (32 per env, 16 per articulation; D
 Neither robot is `mobile`, so gravity on it is off (feeding.py:150-151)."""
 import numpy as np
 
-from .feeding_batch import HEAD_LINK, TREMOR_JOINTS, FeedingBatch
+from . import toc
+from .feeding_batch import TREMOR_JOINTS, FeedingBatch
 from .human_model import create_human
-from .kinematics import BodyKinematics, q_from_rpy, q_rot
+from .kinematics import BodyKinematics, q_from_rpy
 from .scene import SceneBuilder, quat_from_rpy
 from .toc import TocPlacement
 
 MOTOR_POSITION = 1
 
-SAWYER = dict(asset='sawyer', base_pos=[-1, -1, 0.975], load=dict(self_collision=True),
-              arm=[3, 8, 9, 10, 11, 13, 16], ee=19, gripper=[20, 22], tool_joint=18, gripper_collision=[18, 20, 21, 22, 23],
-              gripper_pos=[0.0, 0.0], tool_pos_offset=[-0.1, 0.12, -0.02], tool_orient_offset=[np.pi / 2.0 - 0.1, 0, np.pi / 2.0],
-              toc_base_pos_offset=[-0.1, 0.2, 0.975], ee_orient_rpy=[np.pi / 2.0, 0, np.pi / 2.0], weld_preset={}, default_q=None)
-PR2 = dict(asset='pr2', base_pos=[-1, -1, 0], load=dict(inertia_from_file=True),
-           arm=[42, 43, 44, 46, 47, 49, 50], ee=54, gripper=[57, 58, 59, 60], tool_joint=54, gripper_collision=list(range(49, 64)),
-           gripper_pos=[0.03] * 4, tool_pos_offset=[0, -0.03, -0.11], tool_orient_offset=[-0.2, 0, 0],
-           toc_base_pos_offset=[0.1, 0.2, 0], ee_orient_rpy=[np.pi / 2.0, 0, 0],
-           weld_preset=dict(zip([64, 65, 66, 68, 69, 71, 72], [1.75, 1.25, 1.5, -0.5, 1, 0, 1])),
-           default_q=[-1.75, 1.25, -1.5, -0.5, -1, 0, -1])
+SAWYER = dict(toc.SAWYER, gripper_pos=[0.0, 0.0], tool_pos_offset=[-0.1, 0.12, -0.02], tool_orient_offset=[np.pi / 2.0 - 0.1, 0, np.pi / 2.0],
+              toc_base_pos_offset=[-0.1, 0.2, 0.975], ee_orient_rpy=[np.pi / 2.0, 0, np.pi / 2.0])
+PR2 = dict(toc.PR2_RIGHT, gripper_pos=[0.03] * 4, tool_pos_offset=[0, -0.03, -0.11], tool_orient_offset=[-0.2, 0, 0],
+           toc_base_pos_offset=[0.1, 0.2, 0], ee_orient_rpy=[np.pi / 2.0, 0, 0])
 TARGET_EE_POS = np.array([-0.15, -0.65, 1.15])       # feeding.py:139
 
 
@@ -47,16 +42,7 @@ class FeedingTocBatch(TocPlacement, FeedingBatch):
         self.builder = b
         b.set_gravity([0, 0, -9.81])
         self.plane = b.load_urdf('plane')
-        self.robot = b.load_urdf(R['asset'], base_pos=R['base_pos'], fixed_base=True, **R['load'])
-        if R['asset'] == 'sawyer':                       # sawyer.py:55-61
-            for i in range(3, 24):
-                for j in range(3, 24):
-                    b.set_collision_filter_pair(self.robot, self.robot, i, j, False)
-            for i in range(0, 3):
-                for j in range(0, 9):
-                    b.set_collision_filter_pair(self.robot, self.robot, i, j, False)
-        b.weld_joints(self.robot, set(R['arm']) | set(R['gripper']), R['weld_preset'])
-        b.continuous_limits_for_ik(self.robot, R['arm'])
+        self.load_robot(b)
         self.humans = {}
         for gender, z in (('male', 0.89), ('female', 0.86)):
             hb, info = create_human(b, gender=gender, static=True)
@@ -84,19 +70,9 @@ class FeedingTocBatch(TocPlacement, FeedingBatch):
         b.set_gravity([0, 0, 0], body=self.tool)
         self.scene = b.finalize()
         sc = self.scene
-        self.gl = lambda body, link: int(sc['body_link0'][body]) + 1 + link
-        self.arm_links = [self.gl(self.robot, j) for j in R['arm']]
-        self.gripper_links = [self.gl(self.robot, j) for j in R['gripper']]
-        self.ee_link = self.gl(self.robot, R['ee'])
-        self.kin = BodyKinematics(sc, self.robot)
-        self.arm_lower = sc['link_lower'][self.arm_links].copy()
-        self.arm_upper = sc['link_upper'][self.arm_links].copy()
-        nolimit = sc['link_haslimit'][self.arm_links] == 0
-        self.arm_lower[nolimit], self.arm_upper[nolimit] = -1e10, 1e10
+        self.robot_links(sc)
         self.hkin = {g: BodyKinematics(sc, hb) for g, hb in self.humans.items()}
         self.mouth = {'male': np.array([0, -0.11, 0.03]), 'female': np.array([0, -0.1, 0.03])}
-        self.robot_base_pos = np.array(R['base_pos'], dtype=np.float64)
-        self.robot_base_quat = np.array([0, 0, 0, 1.0])
         self.obstacles = (self.humans['male'], self.humans['female'], self.table, self.wheelchair)     # env.py:300-309
 
     def reset(self, sim, rng, settle_steps=25, sample=None, impairment='random', simulate_head=False, attempts=50, max_iterations=3):
@@ -109,17 +85,6 @@ class FeedingTocBatch(TocPlacement, FeedingBatch):
         sp = self._reset_toc_robot(sim, s, rng, attempts, max_iterations)
         self._reset_bowl_food(sim, s, sp, settle_steps)
         return s
-
-    def mouth_target(self, sim, male):
-        """generate_target (feeding.py:185-190): the mouth offset in the active person's head frame."""
-        sim.forward_kinematics()
-        out = np.zeros((sim.n, 3))
-        for g, hb in self.humans.items():
-            on = male if g == 'male' else ~male
-            st = sim.get_link_states([self.gl(hb, HEAD_LINK)])
-            hp, hq = st['pos'][:, 0].astype(np.float64), st['quat'][:, 0].astype(np.float64)
-            out[on] = (hp + q_rot(hq, np.broadcast_to(self.mouth[g], hp.shape)))[on]
-        return out
 
     def _reset_toc_robot(self, sim, s, rng, attempts, max_iterations):
         n, R = sim.n, self.R

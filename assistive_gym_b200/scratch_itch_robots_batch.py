@@ -17,24 +17,19 @@ With the person's right arm in both genders (2 x 10) that is 29 and 31 DoF per e
 off (scratch_itch.py:123-126), as on the person and the scratcher."""
 import numpy as np
 
-from .dressing_batch import PR2 as DRESS_PR2
+from . import toc
 from .human_model import create_human
-from .kinematics import BodyKinematics, q_from_rpy
+from .kinematics import q_from_rpy
 from .scene import SceneBuilder, quat_from_rpy
 from .scratch_itch_batch import R_ELBOW, R_SHOULDER, R_WRIST, RIGHT_ARM_JOINTS, ScratchItchBatch
 from .toc import TocPlacement
 
 MOTOR_POSITION = 1
 
-SAWYER = dict(asset='sawyer', base_pos=[-1, -1, 0.975], load=dict(self_collision=True),
-              arm=[3, 8, 9, 10, 11, 13, 16], ee=19, gripper=[20, 22], tool_joint=18, gripper_collision=[18, 20, 21, 22, 23],
-              gripper_pos=[0.015, -0.015], tool_pos_offset=[0, 0.125, 0], tool_orient_offset=[0, 0, np.pi / 2.0],
-              toc_base_pos_offset=[-0.1, 0, 0.975], ee_orient_rpy=[0, np.pi / 2.0, 0], weld_preset={}, default_q=None)
-PR2 = dict(asset='pr2', base_pos=[-1, -1, 0], load=dict(inertia_from_file=True),
-           arm=DRESS_PR2['arm'], ee=76, gripper=DRESS_PR2['gripper'], tool_joint=76, gripper_collision=list(range(71, 86)),
-           gripper_pos=[0.25] * 4, tool_pos_offset=[0, 0, 0], tool_orient_offset=[0, 0, 0],
-           toc_base_pos_offset=[0.1, 0, 0], ee_orient_rpy=[0, 0, 0],
-           weld_preset=dict(zip(DRESS_PR2['right_arm'], DRESS_PR2['right_preset'])), default_q=DRESS_PR2['left_preset'])
+SAWYER = dict(toc.SAWYER, gripper_pos=[0.015, -0.015], tool_pos_offset=[0, 0.125, 0], tool_orient_offset=[0, 0, np.pi / 2.0],
+              toc_base_pos_offset=[-0.1, 0, 0.975], ee_orient_rpy=[0, np.pi / 2.0, 0])
+PR2 = dict(toc.PR2_LEFT, gripper_pos=[0.25] * 4, tool_pos_offset=[0, 0, 0], tool_orient_offset=[0, 0, 0],
+           toc_base_pos_offset=[0.1, 0, 0], ee_orient_rpy=[0, 0, 0])
 TARGET_EE_POS = np.array([-0.6, 0, 0.8])             # scratch_itch.py:114
 
 
@@ -49,16 +44,7 @@ class ScratchItchTocBatch(TocPlacement, ScratchItchBatch):
         self.builder = b
         b.set_gravity([0, 0, -9.81])
         self.plane = b.load_urdf('plane')
-        self.robot = b.load_urdf(R['asset'], base_pos=R['base_pos'], fixed_base=True, **R['load'])
-        if R['asset'] == 'sawyer':                       # sawyer.py:55-61
-            for i in range(3, 24):
-                for j in range(3, 24):
-                    b.set_collision_filter_pair(self.robot, self.robot, i, j, False)
-            for i in range(0, 3):
-                for j in range(0, 9):
-                    b.set_collision_filter_pair(self.robot, self.robot, i, j, False)
-        b.weld_joints(self.robot, set(R['arm']) | set(R['gripper']), R['weld_preset'])
-        b.continuous_limits_for_ik(self.robot, R['arm'])
+        self.load_robot(b)
         self.humans = {}
         for gender, z in (('male', 0.89), ('female', 0.86)):
             hb, info = create_human(b, gender=gender, static=True)
@@ -80,18 +66,8 @@ class ScratchItchTocBatch(TocPlacement, ScratchItchBatch):
         b.set_gravity([0, 0, 0], body=self.tool)
         self.scene = b.finalize()
         sc = self.scene
-        self.gl = lambda body, link: int(sc['body_link0'][body]) + 1 + link
-        self.arm_links = [self.gl(self.robot, j) for j in R['arm']]
-        self.gripper_links = [self.gl(self.robot, j) for j in R['gripper']]
-        self.ee_link = self.gl(self.robot, R['ee'])
-        self.kin = BodyKinematics(sc, self.robot)
-        self.arm_lower = sc['link_lower'][self.arm_links].copy()
-        self.arm_upper = sc['link_upper'][self.arm_links].copy()
-        nolimit = sc['link_haslimit'][self.arm_links] == 0
-        self.arm_lower[nolimit], self.arm_upper[nolimit] = -1e10, 1e10
+        self.robot_links(sc)
         self.human_arm_links = {g: [self.gl(hb, j) for j in RIGHT_ARM_JOINTS] for g, hb in self.humans.items()}
-        self.robot_base_pos = np.array(R['base_pos'], dtype=np.float64)
-        self.robot_base_quat = np.array([0, 0, 0, 1.0])
         self.obstacles = (self.humans['male'], self.humans['female'], self.wheelchair)      # collision_objects of scratch_itch.py:116
 
     def reset(self, sim, rng, sample=None, attempts=50, max_iterations=3):

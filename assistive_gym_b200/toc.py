@@ -6,7 +6,23 @@ number of goals reached, ties by the sum over reached goals of the joint-limited
 arm Jacobian at the IK solution; a pose whose start goal is unreachable is discarded."""
 import numpy as np
 
-from .kinematics import q_mul, q_rot
+from .kinematics import BodyKinematics, q_mul, q_rot
+
+# The robots' own constants, the same for every task (agents/sawyer.py and agents/pr2.py): URDF and load pose, the simulated arm
+# and gripper joints of the arm that holds the tool, the end effector and tool joint, the gripper links that ignore the tool, and
+# the angles of the joints that are welded.  PR2 with the right arm welds its left arm at the angles `reset_joints` gives it
+# (pr2.py:60-66) and starts the TOC search from the right arm's; with the left arm the other way round.
+SAWYER = dict(asset='sawyer', base_pos=[-1, -1, 0.975], load=dict(self_collision=True),
+              arm=[3, 8, 9, 10, 11, 13, 16], ee=19, gripper=[20, 22], tool_joint=18, gripper_collision=[18, 20, 21, 22, 23],
+              weld_preset={}, default_q=None)
+_PR2_RIGHT_ARM, _PR2_LEFT_ARM = [42, 43, 44, 46, 47, 49, 50], [64, 65, 66, 68, 69, 71, 72]
+_PR2_RIGHT_PRESET, _PR2_LEFT_PRESET = [-1.75, 1.25, -1.5, -0.5, -1, 0, -1], [1.75, 1.25, 1.5, -0.5, 1, 0, 1]
+PR2_RIGHT = dict(asset='pr2', base_pos=[-1, -1, 0], load=dict(inertia_from_file=True),
+                 arm=_PR2_RIGHT_ARM, ee=54, gripper=[57, 58, 59, 60], tool_joint=54, gripper_collision=list(range(49, 64)),
+                 weld_preset=dict(zip(_PR2_LEFT_ARM, _PR2_LEFT_PRESET)), default_q=_PR2_RIGHT_PRESET)
+PR2_LEFT = dict(asset='pr2', base_pos=[-1, -1, 0], load=dict(inertia_from_file=True),
+                arm=_PR2_LEFT_ARM, ee=76, gripper=[79, 80, 81, 82], tool_joint=76, gripper_collision=list(range(71, 86)),
+                weld_preset=dict(zip(_PR2_RIGHT_ARM, _PR2_RIGHT_PRESET)), default_q=_PR2_LEFT_PRESET)
 
 
 def joint_limited_weighting(q, lower, upper):                    # robot.py:223-235
@@ -81,7 +97,38 @@ class TocPlacement:
     """`init_robot_pose`'s TOC branch (env.py:276-310) for a batched scene whose robot is not wheelchair-mounted: a TOC search,
     then a collision check of robot and tool against `obstacles`, re-searching only the colliding envs for up to `max_iterations`
     rounds.  The scene class provides `R` (the robot's task constants), `robot`, `tool`, `kin`, `arm_links`, `gripper_links`,
-    `ee_link`, `arm_lower`, `arm_upper`, `tool_pos_offset`, `tool_quat_offset` and `obstacles`."""
+    `ee_link`, `arm_lower`, `arm_upper`, `tool_pos_offset`, `tool_quat_offset` and `obstacles`; `load_robot` and `robot_links`
+    set the robot's part of these."""
+
+    def load_robot(self, b):
+        """Load the robot of `R` into the scene builder `b` and weld every joint but the arm and the gripper."""
+        R = self.R
+        self.robot = b.load_urdf(R['asset'], base_pos=R['base_pos'], fixed_base=True, **R['load'])
+        if R['asset'] == 'sawyer':                       # sawyer.py:55-61
+            for i in range(3, 24):
+                for j in range(3, 24):
+                    b.set_collision_filter_pair(self.robot, self.robot, i, j, False)
+            for i in range(0, 3):
+                for j in range(0, 9):
+                    b.set_collision_filter_pair(self.robot, self.robot, i, j, False)
+        b.weld_joints(self.robot, set(R['arm']) | set(R['gripper']), R['weld_preset'])
+        b.continuous_limits_for_ik(self.robot, R['arm'])
+
+    def robot_links(self, sc):
+        """The robot's links in the finalised scene `sc`: `gl`, arm, gripper and end-effector links, its kinematics, the arm's
+        limits (+-1e10 for unlimited joints) and its load pose."""
+        R = self.R
+        self.gl = lambda body, link: int(sc['body_link0'][body]) + 1 + link
+        self.arm_links = [self.gl(self.robot, j) for j in R['arm']]
+        self.gripper_links = [self.gl(self.robot, j) for j in R['gripper']]
+        self.ee_link = self.gl(self.robot, R['ee'])
+        self.kin = BodyKinematics(sc, self.robot)
+        self.arm_lower = sc['link_lower'][self.arm_links].copy()
+        self.arm_upper = sc['link_upper'][self.arm_links].copy()
+        nolimit = sc['link_haslimit'][self.arm_links] == 0
+        self.arm_lower[nolimit], self.arm_upper[nolimit] = -1e10, 1e10
+        self.robot_base_pos = np.array(R['base_pos'], dtype=np.float64)
+        self.robot_base_quat = np.array([0, 0, 0, 1.0])
 
     def place_robot(self, sim, base_pos, base_quat, q7):
         """Robot base, arm, open gripper and the tool at the tool joint's COM frame composed with the offsets (tool.py:49-54);
@@ -91,6 +138,9 @@ class TocPlacement:
         sim.set_base_velocity(self.robot, np.zeros((n, 3)), np.zeros((n, 3)))
         sim.set_joint_state(self.arm_links, q=q7, qd=np.zeros_like(q7))
         gq = np.tile(R['gripper_pos'], (n, 1)).astype(np.float64)
+        # set_instantly clips to the joint limits (set_joint_angles(use_limits=True)): Sawyer's drinking opening of 0.025 lands at 0.020833
+        sc = self.scene
+        gq = np.clip(gq, sc['link_lower'][self.gripper_links], sc['link_upper'][self.gripper_links])
         sim.set_joint_state(self.gripper_links, q=gq, qd=np.zeros_like(gq))
         qfull = np.zeros((n, self.kin.nl))
         qfull[:, np.array(R['arm']) + 1] = q7

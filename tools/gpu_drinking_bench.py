@@ -1,12 +1,13 @@
 #!/usr/bin/env python3
-"""GPU box: DrinkingJaco-v1 fused step throughput (ag_drinking_step_*), device-timed; not the headline metric.
+"""GPU box: fused Drinking step throughput (ag_drinking_step_*), device-timed; not the headline metric.
 
 One JSON line: the card and its power limit (read in the same run), reset time, the graph-replayed device step
 (`drinking_step_dev`, CUDA events) and the host-buffer step (`drinking_step_host`, host clock; the call ends in a stream
 synchronise) over the same number of steps after a warm-up, a per-kernel split from a separate profiled pass, contacts and PGS
-iterations per env, overflowed envs and the sim's device memory.
+iterations per env, overflowed envs and the sim's device memory.  With `--ids` one line per id (DrinkingJaco-v1, DrinkingSawyer-v1,
+DrinkingPR2-v1; the TOC ids also report the envs their placement left colliding).
 
-usage: python tools/gpu_drinking_bench.py [--n 4096] [--steps 100] [--warmup 10] [--profile-steps 5] [--out FILE]"""
+usage: python tools/gpu_drinking_bench.py [--ids DrinkingJaco-v1,...] [--n 4096] [--steps 100] [--warmup 10] [--profile-steps 5] [--out FILE]"""
 import argparse
 import json
 import os
@@ -19,7 +20,8 @@ sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
-from assistive_gym_b200.drinking_batch import DrinkingBatch  # noqa: E402
+from assistive_gym_b200.envs import ENV_REGISTRY  # noqa: E402
+from assistive_gym_b200.envs.drinking import drinking_batch_for  # noqa: E402
 from assistive_gym_b200.sim import BatchSim  # noqa: E402
 
 
@@ -32,6 +34,7 @@ def gpu_info():
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument('--ids', default='DrinkingJaco-v1', help='comma-separated Drinking ids, one JSON line each')
     ap.add_argument('--n', type=int, default=4096)
     ap.add_argument('--steps', type=int, default=100)
     ap.add_argument('--warmup', type=int, default=10)
@@ -40,12 +43,19 @@ def main():
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit('no CUDA device: this measurement needs the GPU')
+    lines = [bench(env_id, args) for env_id in args.ids.split(',')]
+    if args.out:
+        with open(args.out, 'w') as f:
+            f.write(''.join(line + '\n' for line in lines))
+
+
+def bench(env_id, args):
     n, K, W = args.n, args.steps, args.warmup
     gpu = gpu_info()
-    db = DrinkingBatch()
+    db = drinking_batch_for(ENV_REGISTRY[env_id]().robot)
     torch.cuda.synchronize()
     free0 = torch.cuda.mem_get_info()[0]
-    sim = BatchSim(db.scene, DrinkingBatch.config(), n)
+    sim = BatchSim(db.scene, db.config(), n)
     t0 = time.time()
     s = db.reset(sim, np.random.default_rng(0), settle_steps=50, impairment='no_tremor')
     db.start_fused(sim, s)
@@ -92,7 +102,7 @@ def main():
     kernels = {k: {'ms_per_step': ms / args.profile_steps, 'launches_per_step': c / args.profile_steps, 'share': ms / total}
                for k, (ms, c) in sorted(prof.items(), key=lambda kv: -kv[1][0])}
     overflow = sim.overflow_count()
-    out = {'workload': 'DrinkingJaco-v1 fused step', 'gpu': gpu, 'n_envs': n, 'steps': K, 'warmup': W,
+    out = {'workload': '%s fused step' % env_id, 'gpu': gpu, 'n_envs': n, 'steps': K, 'warmup': W,
            'num_substeps': 4, 'frame_skip': 5, 'num_solver_iters': 10, 'max_contacts': 512,
            'reset_s': reset_s, 'device_step_ms': dev_ms, 'device_env_steps_per_s': n / dev_ms * 1e3,
            'host_step_ms': host_ms, 'host_env_steps_per_s': n / host_ms * 1e3,
@@ -100,12 +110,12 @@ def main():
            'overflow_envs_reset': overflow_reset, 'overflow_envs_steps': overflow, 'sim_device_bytes': int(sim_bytes),
            'particles_in_play_mean': float(in_play.mean()), 'task_success_mean': float(ts.mean()), 'finite': finite,
            'profiled_steps': args.profile_steps, 'profiled_ms_per_step': total / args.profile_steps, 'kernels': kernels}
+    if hasattr(db, 'unresolved'):
+        out['toc_envs_left_colliding'] = int(db.unresolved)
     line = json.dumps(out)
-    print(line)
-    if args.out:
-        with open(args.out, 'w') as f:
-            f.write(line + '\n')
+    print(line, flush=True)
     sim.close()
+    return line
 
 
 if __name__ == '__main__':
