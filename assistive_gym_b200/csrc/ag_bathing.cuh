@@ -4,8 +4,7 @@
 // With a controllable person (BedBathingSawyerHuman-v1, run by ag_coop.cuh) the right arm moves, and bathing_track_body
 // re-places every target on its upper-arm / forearm link (update_targets, bed_bathing.py:190-203).
 #pragma once
-#include "ag_device.cuh"
-#include "ag_feeding.cuh"
+#include "ag_task.cuh"
 #include "../../include/agphys.h"
 
 struct BathDev {
@@ -23,24 +22,10 @@ struct BathDev {
 // action -> PD targets (env.py:187-217), same accumulate-with-limit-clamp rule as the feeding path.
 // p0 = action [N][7 + i0] (env-major; the robot's 7 come first), p1 = BathDev*
 AG_HDN inline void bathing_pre_body(int e, const SimDev& S, const KP& p) {
-  const int N = S.N;
   const BathDev& B = *(const BathDev*)p.p1;
   const float* act = (const float*)p.p0 + (size_t)e * (7 + p.i0);
   B.iteration[e] += 1;
-  for (int j = 0; j < 7; j++) {
-    float raw = act[j];
-    B.action[(size_t)j * N + e] = raw;
-    float a = clampf(raw, -1.f, 1.f) * B.P.action_multiplier;
-    int k = B.P.arm_links[j];
-    float q = ld1(S.jq, k, N, e);
-    float lo = B.P.arm_lower[j], hi = B.P.arm_upper[j];
-    for (int s = 0; s < B.P.frame_skip; s++) {
-      if (q + a < lo) { a = 0.f; q = lo; }
-      if (q + a > hi) { a = 0.f; q = hi; }
-      q += a;
-    }
-    st1(S.motor_target, k, N, e, q);
-  }
+  arm_action_targets(S, e, act, B.action, B.P.arm_links, B.P.arm_lower, B.P.arm_upper, B.P.action_multiplier, B.P.frame_skip);
 }
 
 // thread = (collider slot of the person, env): distance from that collider to the nearest wiper collider,
@@ -85,49 +70,30 @@ AG_HDN inline void bathing_post_body(int e, const SimDev& S, const KP& p) {
   const AgBathingParams& P = B.P;
   bool male = B.male[e] != 0;
   int hb = male ? P.human_body_m : P.human_body_f;
-  int lr = AG_LDG(S.body_link0 + P.robot_body);
-  // robot base pose = its inertial frame, as p.getBasePositionAndOrientation reports it (agent.py:49,58-63)
-  q4 rq = ld4(S.lquat, lr, N, e);
-  f3 rp = ld3(S.lpos, lr, N, e) + qrot(rq, tv3(S.link_com, lr));
-  rq = qmul(rq, tv4(S.link_iquat, lr));
-  q4 rqi = qconj(rq);
+  Frame fr = body_frame(S, e, P.robot_body);
   // tool link 1 (the cloth) link-frame pose in the robot frame (bed_bathing.py:81-82)
   f3 tp = ld3(S.lpos, P.cloth_link, N, e); q4 tq = ld4(S.lquat, P.cloth_link, N, e);
-  f3 tp_r = qrot(rqi, tp - rp); q4 tq_r = qmul(rqi, tq);
   float* obs = (float*)p.p2 + (size_t)e * 24;
-  obs[0] = tp_r.x; obs[1] = tp_r.y; obs[2] = tp_r.z; obs[3] = tq_r.x; obs[4] = tq_r.y; obs[5] = tq_r.z; obs[6] = tq_r.w;
-  const float PI = 3.14159265358979323846f;
-  for (int j = 0; j < 7; j++) {
-    float q = ld1(S.jq, P.arm_links[j], N, e) + PI;
-    obs[7 + j] = q - 2.f * PI * floorf(q / (2.f * PI)) - PI;
-  }
-  for (int j = 0; j < 3; j++) {      // shoulder, elbow, wrist link positions in the robot frame
-    int k = male ? P.arm_points_m[j] : P.arm_points_f[j];
-    f3 q = qrot(rqi, ld3(S.lpos, k, N, e) - rp);
-    obs[14 + 3 * j] = q.x; obs[15 + 3 * j] = q.y; obs[16 + 3 * j] = q.z;
-  }
+  int o = put3(obs, 0, to_frame(fr, tp)); o = put4(obs, o, to_frame(fr, tq));
+  o = put_arm_angles(S, e, P.arm_links, obs, o);
+  o = put_arm_points(S, e, fr, male ? P.arm_points_m : P.arm_points_f, obs, o);
   // forces and wiped targets (bed_bathing.py:41-78)
   float tool_force = 0.f, tool_on_human = 0.f, total_on_human = 0.f;
   int new_pts = 0;
-  int cnt = S.c_count[e]; if (cnt > S.maxc) cnt = S.maxc;
+  int cnt = n_contacts(S, e);
   const int T = P.n_targets_max;
   for (int s = 0; s < cnt; s++) {
-    unsigned pk = S.s_key[(size_t)s * N + e] >> 2;
-    int ca = (int)(pk / (unsigned)S.nc), cb = (int)(pk % (unsigned)S.nc);
-    int la = AG_LDG(S.col_link + ca), lb = AG_LDG(S.col_link + cb);
-    int ba = AG_LDG(S.link_body + la), bb = AG_LDG(S.link_body + lb);
-    float force = cf_ld(S.s_data, s, CF_LAM_N, N, e) / S.dt;
-    if (ba == P.tool_body || bb == P.tool_body) tool_force += force;
-    bool a_h = ba == hb, b_h = bb == hb;
-    if (!a_h && !b_h) continue;
-    int other = a_h ? bb : ba, lo = a_h ? lb : la;
+    Contact c = contact_at(S, e, s);
+    float force = contact_force(S, e, s);
+    if (c.ba == P.tool_body || c.bb == P.tool_body) tool_force += force;
+    int other, lo;
+    if (!other_of(c, hb, other, lo)) continue;
     if (other == P.robot_body) total_on_human += force;
     else if (other == P.tool_body) {
       total_on_human += force;
       if (lo != P.cloth_link) continue;
       tool_on_human += force;
-      f3 ph = a_h ? f3(cf_ld(S.s_data, s, CF_PAX, N, e), cf_ld(S.s_data, s, CF_PAY, N, e), cf_ld(S.s_data, s, CF_PAZ, N, e))
-                  : f3(cf_ld(S.s_data, s, CF_PBX, N, e), cf_ld(S.s_data, s, CF_PBY, N, e), cf_ld(S.s_data, s, CF_PBZ, N, e));
+      f3 ph = contact_point_on(S, e, s, c, hb);
       for (int t = 0; t < T; t++) {
         if (!B.alive[(size_t)t * N + e]) continue;
         f3 tw = ld3(B.targets, t, N, e);
@@ -135,20 +101,16 @@ AG_HDN inline void bathing_post_body(int e, const SimDev& S, const KP& p) {
       }
     }
   }
-  obs[23] = tool_force;
+  obs[o] = tool_force;
   int success = B.task_success[e] + new_pts;
   B.task_success[e] = success;
   float dmin = 5.0f;
   for (int i = 0; i < B.n_slots; i++) dmin = fminf(dmin, B.dist_part[(size_t)i * N + e]);
-  f3 eecom = ld3(S.lpos, P.ee_link, N, e) + qrot(ld4(S.lquat, P.ee_link, N, e), tv3(S.link_com, P.ee_link));
-  f3 lin, ang; link_velocity(S, e, P.ee_link, eecom, lin, ang);
   // human preferences (env.py:237-274), task == 'bed_bathing'
-  float pref = P.c_v * (-norm(lin)) + P.c_f * (-(total_on_human - tool_on_human)) + P.c_hf * (tool_on_human < 10.f ? 0.f : -tool_on_human);
-  float an = 0.f;
-  for (int j = 0; j < 7; j++) { float a = B.action[(size_t)j * N + e]; an += a * a; }
-  for (int j = 0; j < p.i0; j++) { float a = ((const float*)p.p0)[(size_t)e * (7 + p.i0) + 7 + j]; an += a * a; }
-  ((float*)p.p3)[e] = P.w_distance * (-dmin) + P.w_action * (-sqrtf(an)) + P.w_wiping * (float)new_pts + pref;
-  ((float*)p.p4)[e] = B.iteration[e] >= 200 ? 1.f : 0.f;
+  float pref = P.c_v * (-ee_speed(S, e, P.ee_link)) + P.c_f * (-(total_on_human - tool_on_human)) + P.c_hf * (tool_on_human < 10.f ? 0.f : -tool_on_human);
+  float an = action_norm(S, e, B.action, (const float*)p.p0, p.i0);
+  ((float*)p.p3)[e] = P.w_distance * (-dmin) + P.w_action * (-an) + P.w_wiping * (float)new_pts + pref;
+  ((float*)p.p4)[e] = episode_done(B.iteration[e]);
   float* info = (float*)p.p5 + (size_t)e * 4;
   info[0] = total_on_human; info[1] = ((float)success >= (float)B.total_targets[e] * P.task_success_threshold) ? 1.f : 0.f;
   info[2] = tool_on_human; info[3] = (float)new_pts;

@@ -19,7 +19,7 @@
 // in the layer order of limits_model.ArmLimitsModel.predict.
 #pragma once
 #include <math.h>
-#include "ag_device.cuh"
+#include "ag_task.cuh"
 #include "ag_bathing.cuh"
 #include "ag_dressing.cuh"
 #include "ag_feeding.cuh"
@@ -139,17 +139,6 @@ AG_HDN inline void coop_limits_body(int e, const SimDev& S, const CoopDev& C, co
   }
 }
 
-// the person's base frame = its inertial frame (p.getBasePositionAndOrientation, agent.py:49,58-63)
-AG_HD void coop_base_frame(const SimDev& S, int e, int body, f3& bp, q4& bqi) {
-  const int N = S.N;
-  const int l0 = AG_LDG(S.body_link0 + body);
-  q4 q = ld4(S.lquat, l0, N, e);
-  bp = ld3(S.lpos, l0, N, e) + qrot(q, tv3(S.link_com, l0));
-  bqi = qconj(qmul(q, tv4(S.link_iquat, l0)));
-}
-AG_HD int coop_put3(float* o, int i, f3 v) { o[i] = v.x; o[i + 1] = v.y; o[i + 2] = v.z; return i + 3; }
-AG_HD int coop_put4(float* o, int i, q4 v) { o[i] = v.x; o[i + 1] = v.y; o[i + 2] = v.z; o[i + 3] = v.w; return i + 4; }
-
 // p1 = CoopDev*, p2 = FeedDev* | ScratchDev* | BathDev* | DressPost*, p3 = obs_human [N][23 | 34 | 28 | 28], p4 = info [N][4]
 // written by the task's post kernel
 AG_HDN inline void coop_obs_body(int e, const SimDev& S, const KP& p) {
@@ -158,63 +147,46 @@ AG_HDN inline void coop_obs_body(int e, const SimDev& S, const KP& p) {
   const AgCoopParams& P = C.P;
   const bool male = C.male[e] != 0;
   const int* links = male ? P.joint_links_m : P.joint_links_f;
-  f3 bp; q4 bqi;
-  coop_base_frame(S, e, male ? P.human_body_m : P.human_body_f, bp, bqi);
+  const Frame fr = body_frame(S, e, male ? P.human_body_m : P.human_body_f);      // the person's base frame
   const float* info = (const float*)p.p4 + (size_t)e * 4;
   int i = 0;
   if (P.task == 0) {                          // feeding.py:101-111
     const FeedDev& F = *(const FeedDev*)p.p2;
-    const int ltool = AG_LDG(S.body_link0 + F.P.tool_body), head = male ? F.P.head_link_m : F.P.head_link_f;
-    q4 tq = ld4(S.lquat, ltool, N, e);
-    f3 sp = ld3(S.lpos, ltool, N, e) + qrot(tq, tv3(S.link_com, ltool));
-    q4 sq = qmul(tq, tv4(S.link_iquat, ltool));
-    f3 hp = ld3(S.lpos, head, N, e); q4 hq = ld4(S.lquat, head, N, e);
-    f3 mouth = male ? f3(F.P.mouth_m[0], F.P.mouth_m[1], F.P.mouth_m[2]) : f3(F.P.mouth_f[0], F.P.mouth_f[1], F.P.mouth_f[2]);
-    f3 target = hp + qrot(hq, mouth);
+    f3 sp, hp; q4 sq, hq;
+    link_com_pose(S, e, AG_LDG(S.body_link0 + F.P.tool_body), sp, sq);
+    f3 target = mouth_target(S, e, male ? F.P.head_link_m : F.P.head_link_f, male ? F.P.mouth_m : F.P.mouth_f, hp, hq);
     float* o = (float*)p.p3 + (size_t)e * 23;
-    f3 sp_h = qrot(bqi, sp - bp), tg_h = qrot(bqi, target - bp);
-    i = coop_put3(o, i, sp_h); i = coop_put4(o, i, qmul(bqi, sq)); i = coop_put3(o, i, sp_h - tg_h);
+    f3 sp_h = to_frame(fr, sp), tg_h = to_frame(fr, target);
+    i = put3(o, i, sp_h); i = put4(o, i, to_frame(fr, sq)); i = put3(o, i, sp_h - tg_h);
     for (int c = 0; c < P.n_ctrl; c++) o[i++] = ld1(S.jq, links[P.ctrl[c]], N, e);
-    i = coop_put3(o, i, qrot(bqi, hp - bp)); i = coop_put4(o, i, qmul(bqi, hq));
+    i = put3(o, i, to_frame(fr, hp)); i = put4(o, i, to_frame(fr, hq));
     o[i++] = info[2];                         // robot force on the person
     o[i++] = info[3];                         // spoon force on the person
   } else if (P.task == 2) {                   // bed_bathing.py:97-105
     const BathDev& B = *(const BathDev*)p.p2;
-    f3 tp = ld3(S.lpos, B.P.cloth_link, N, e); q4 tq = ld4(S.lquat, B.P.cloth_link, N, e);
     float* o = (float*)p.p3 + (size_t)e * 28;
-    i = coop_put3(o, i, qrot(bqi, tp - bp)); i = coop_put4(o, i, qmul(bqi, tq));
+    i = put3(o, i, to_frame(fr, ld3(S.lpos, B.P.cloth_link, N, e))); i = put4(o, i, to_frame(fr, ld4(S.lquat, B.P.cloth_link, N, e)));
     for (int c = 0; c < P.n_ctrl; c++) o[i++] = ld1(S.jq, links[P.ctrl[c]], N, e);
-    for (int j = 0; j < 3; j++) {
-      const int k = male ? B.P.arm_points_m[j] : B.P.arm_points_f[j];
-      i = coop_put3(o, i, qrot(bqi, ld3(S.lpos, k, N, e) - bp));
-    }
+    i = put_arm_points(S, e, fr, male ? B.P.arm_points_m : B.P.arm_points_f, o, i);
     o[i++] = info[0];                         // total force on the person
     o[i++] = info[2];                         // wiper-cloth force on the person
   } else if (P.task == 3) {                   // dressing.py:96-105
     const DressDev& D = ((const DressPost*)p.p2)->D;
-    f3 ep = ld3(S.lpos, D.P.ee_link, N, e); q4 eq = ld4(S.lquat, D.P.ee_link, N, e);
     float* o = (float*)p.p3 + (size_t)e * 28;
-    i = coop_put3(o, i, qrot(bqi, ep - bp)); i = coop_put4(o, i, qmul(bqi, eq));
+    i = put3(o, i, to_frame(fr, ld3(S.lpos, D.P.ee_link, N, e))); i = put4(o, i, to_frame(fr, ld4(S.lquat, D.P.ee_link, N, e)));
     for (int c = 0; c < P.n_ctrl; c++) o[i++] = ld1(S.jq, links[P.ctrl[c]], N, e);
-    for (int j = 0; j < 3; j++) {
-      const int k = male ? D.P.arm_points_m[j] : D.P.arm_points_f[j];
-      i = coop_put3(o, i, qrot(bqi, ld3(S.lpos, k, N, e) - bp));
-    }
+    i = put_arm_points(S, e, fr, male ? D.P.arm_points_m : D.P.arm_points_f, o, i);
     o[i++] = D.person_force[e];               // cloth force sum (k_dress_post)
     o[i++] = D.person_force[(size_t)N + e];   // robot force on the person
   } else {                                    // scratch_itch.py:75-84
     const ScratchDev& D = *(const ScratchDev*)p.p2;
-    f3 tp = ld3(S.lpos, D.P.tool_tip_link, N, e); q4 tq = ld4(S.lquat, D.P.tool_tip_link, N, e);
     const int limb = D.limb_link[e];
     f3 target = ld3(S.lpos, limb, N, e) + qrot(ld4(S.lquat, limb, N, e), ld3(D.target_local, 0, N, e));
     float* o = (float*)p.p3 + (size_t)e * 34;
-    f3 tp_h = qrot(bqi, tp - bp), tg_h = qrot(bqi, target - bp);
-    i = coop_put3(o, i, tp_h); i = coop_put4(o, i, qmul(bqi, tq)); i = coop_put3(o, i, tp_h - tg_h); i = coop_put3(o, i, tg_h);
+    f3 tp_h = to_frame(fr, ld3(S.lpos, D.P.tool_tip_link, N, e)), tg_h = to_frame(fr, target);
+    i = put3(o, i, tp_h); i = put4(o, i, to_frame(fr, ld4(S.lquat, D.P.tool_tip_link, N, e))); i = put3(o, i, tp_h - tg_h); i = put3(o, i, tg_h);
     for (int c = 0; c < P.n_ctrl; c++) o[i++] = ld1(S.jq, links[P.ctrl[c]], N, e);
-    for (int j = 0; j < 3; j++) {
-      const int k = male ? D.P.arm_points_m[j] : D.P.arm_points_f[j];
-      i = coop_put3(o, i, qrot(bqi, ld3(S.lpos, k, N, e) - bp));
-    }
+    i = put_arm_points(S, e, fr, male ? D.P.arm_points_m : D.P.arm_points_f, o, i);
     o[i++] = info[0];                         // total force on the person
     o[i++] = info[2];                         // tool force at the target
   }

@@ -5,8 +5,7 @@
 // then read action rows of 7 + KP.i0 floats, and the post kernel leaves the two forces of the person's observation in
 // `person_force` for k_coop_obs.
 #pragma once
-#include "ag_device.cuh"
-#include "ag_feeding.cuh"
+#include "ag_task.cuh"
 #include "ag_cloth.cuh"
 #include "../../include/agphys.h"
 
@@ -23,31 +22,12 @@ struct DressDev {
 // action -> PD targets of the robot's 7 arm joints (env.py:187-217).
 // p0 = action [N][7 + i0] (env-major; the robot's 7 come first), p1 = DressPost* (its leading DressDev)
 AG_HDN inline void dressing_pre_body(int e, const SimDev& S, const KP& p) {
-  const int N = S.N;
   const DressDev& D = *(const DressDev*)p.p1;
   const float* act = (const float*)p.p0 + (size_t)e * (7 + p.i0);
   D.iteration[e] += 1;
-  for (int j = 0; j < 7; j++) {
-    float raw = act[j];
-    D.action[(size_t)j * N + e] = raw;
-    float a = clampf(raw, -1.f, 1.f) * D.P.action_multiplier;
-    int k = D.P.arm_links[j];
-    float q = ld1(S.jq, k, N, e);
-    float lo = D.P.arm_lower[j], hi = D.P.arm_upper[j];
-    for (int s = 0; s < D.P.frame_skip; s++) {
-      if (q + a < lo) { a = 0.f; q = lo; }
-      if (q + a > hi) { a = 0.f; q = hi; }
-      q += a;
-    }
-    st1(S.motor_target, k, N, e, q);
-  }
+  arm_action_targets(S, e, act, D.action, D.P.arm_links, D.P.arm_lower, D.P.arm_upper, D.P.action_multiplier, D.P.frame_skip);
   // a tremor human is an agent (env.py:130): its arm targets flip sign around the rest pose every env step (env.py:212-215)
-  if (D.tremor_on[e]) {
-    bool male = D.male[e] != 0;
-    float sgn = (D.iteration[e] % 2 == 0) ? 1.f : -1.f;
-    for (int j = 0; j < 10; j++)
-      st1(S.motor_target, male ? D.P.human_arm_m[j] : D.P.human_arm_f[j], N, e, D.tremor_rest[(size_t)j * N + e] + sgn * D.tremor_amp[(size_t)j * N + e]);
-  }
+  if (D.tremor_on[e]) tremor_targets(S, e, 10, D.male[e] != 0 ? D.P.human_arm_m : D.P.human_arm_f, D.tremor_rest, D.tremor_amp, D.iteration[e]);
 }
 
 AG_HD float dress_sign(float v) { return v > 0.f ? 1.f : (v < 0.f ? -1.f : 0.f); }
@@ -84,32 +64,19 @@ AG_HDN inline void dressing_post_body(int e, const SimDev& S, const KP& p) {
   const AgDressingParams& P = D.P;
   bool male = D.male[e] != 0;
   int hb = male ? P.human_body_m : P.human_body_f;
-  int lr = AG_LDG(S.body_link0 + P.robot_body);
-  q4 rq = ld4(S.lquat, lr, N, e);
-  f3 rp = ld3(S.lpos, lr, N, e) + qrot(rq, tv3(S.link_com, lr));
-  rq = qmul(rq, tv4(S.link_iquat, lr));
-  q4 rqi = qconj(rq);
+  Frame fr = body_frame(S, e, P.robot_body);
   f3 eep = ld3(S.lpos, P.ee_link, N, e); q4 eeq = ld4(S.lquat, P.ee_link, N, e);
-  f3 ep_r = qrot(rqi, eep - rp); q4 eq_r = qmul(rqi, eeq);
   float* obs = (float*)p.p2 + (size_t)e * 24;
-  obs[0] = ep_r.x; obs[1] = ep_r.y; obs[2] = ep_r.z; obs[3] = eq_r.x; obs[4] = eq_r.y; obs[5] = eq_r.z; obs[6] = eq_r.w;
-  const float PI = 3.14159265358979323846f;
-  for (int j = 0; j < 7; j++) {
-    float q = ld1(S.jq, P.arm_links[j], N, e) + PI;
-    obs[7 + j] = q - 2.f * PI * floorf(q / (2.f * PI)) - PI;
-  }
-  f3 limb[3];                        // shoulder, elbow, wrist link positions (dressing.py:20-22)
-  for (int j = 0; j < 3; j++) {
-    limb[j] = ld3(S.lpos, male ? P.arm_points_m[j] : P.arm_points_f[j], N, e);
-    f3 q = qrot(rqi, limb[j] - rp);
-    obs[14 + 3 * j] = q.x; obs[15 + 3 * j] = q.y; obs[16 + 3 * j] = q.z;
-  }
+  int o = put3(obs, 0, to_frame(fr, eep)); o = put4(obs, o, to_frame(fr, eeq));
+  o = put_arm_angles(S, e, P.arm_links, obs, o);
+  const int32_t* arm_points = male ? P.arm_points_m : P.arm_points_f;      // shoulder, elbow, wrist links (dressing.py:20-22)
+  o = put_arm_points(S, e, fr, arm_points, obs, o);
   // ---- sleeve_on_arm_reward (util.py:134-202)
   f3 pts[6];
   const size_t xb = (size_t)e * 3 * C.nnp;
   for (int i = 0; i < 6; i++) { int n = i < 3 ? P.tri1[i] : P.tri2[i - 3]; pts[i] = f3(C.x[xb + n], C.x[xb + C.nnp + n], C.x[xb + 2 * (size_t)C.nnp + n]); }
   float hand_r = male ? P.hand_radius_m : P.hand_radius_f, elbow_r = male ? P.elbow_radius_m : P.elbow_radius_f, shoulder_r = male ? P.shoulder_radius_m : P.shoulder_radius_f;
-  f3 sh = limb[0], el = limb[1], wr = limb[2];
+  f3 sh = ld3(S.lpos, arm_points[0], N, e), el = ld3(S.lpos, arm_points[1], N, e), wr = ld3(S.lpos, arm_points[2], N, e);
   float lwe = norm(wr - el);
   f3 hand_end = wr + (wr - el) * (1.f / lwe) * (hand_r * 2.f);
   f3 elbow_end = el + (el - wr) * (1.f / lwe) * elbow_r;
@@ -139,26 +106,20 @@ AG_HDN inline void dressing_post_body(int e, const SimDev& S, const KP& p) {
     float fn = norm(f);
     if (r[3] < eep.z - 0.05f && fn < 20.f) cloth_sum += fn;
   }
-  obs[23] = cloth_sum;
+  obs[o] = cloth_sum;
   // ---- robot on person (dressing.py:91)
   float robot_on_human = 0.f;
-  int rc = S.c_count[e]; if (rc > S.maxc) rc = S.maxc;
+  int rc = n_contacts(S, e);
   for (int s = 0; s < rc; s++) {
-    unsigned pk = S.s_key[(size_t)s * N + e] >> 2;
-    int ca = (int)(pk / (unsigned)S.nc), cb = (int)(pk % (unsigned)S.nc);
-    int ba = AG_LDG(S.link_body + AG_LDG(S.col_link + ca)), bb = AG_LDG(S.link_body + AG_LDG(S.col_link + cb));
-    if ((ba == P.robot_body && bb == hb) || (bb == P.robot_body && ba == hb)) robot_on_human += cf_ld(S.s_data, s, CF_LAM_N, N, e) / S.dt;
+    Contact c = contact_at(S, e, s);
+    if ((c.ba == P.robot_body && c.bb == hb) || (c.bb == P.robot_body && c.ba == hb)) robot_on_human += contact_force(S, e, s);
   }
-  f3 eecom = eep + qrot(eeq, tv3(S.link_com, P.ee_link));
-  f3 lin, ang; link_velocity(S, e, P.ee_link, eecom, lin, ang);
-  float pref = P.c_v * (-norm(lin)) + P.c_d * (-cloth_sum);          // env.py:237-274 with the dressing arguments
-  float an = 0.f;
-  for (int j = 0; j < 7; j++) { float a = D.action[(size_t)j * N + e]; an += a * a; }
-  for (int j = 0; j < p.i0; j++) { float a = ((const float*)p.p0)[(size_t)e * (7 + p.i0) + 7 + j]; an += a * a; }
-  ((float*)p.p3)[e] = P.w_dressing * reward_dressing + P.w_action * (-sqrtf(an)) + pref;
+  float pref = P.c_v * (-ee_speed(S, e, P.ee_link)) + P.c_d * (-cloth_sum);          // env.py:237-274 with the dressing arguments
+  float an = action_norm(S, e, D.action, (const float*)p.p0, p.i0);
+  ((float*)p.p3)[e] = P.w_dressing * reward_dressing + P.w_action * (-an) + pref;
   float best = D.task_success[e];
   if (reward_dressing > best) { best = reward_dressing; D.task_success[e] = best; }
-  ((float*)p.p4)[e] = D.iteration[e] >= 200 ? 1.f : 0.f;
+  ((float*)p.p4)[e] = episode_done(D.iteration[e]);
   float* info = (float*)p.p5 + (size_t)e * 4;
   info[0] = robot_on_human + cloth_sum; info[1] = best >= P.task_success_threshold ? 1.f : 0.f; info[2] = reward_dressing;
   info[3] = (forearm_in ? 1.f : 0.f) + (upperarm_in ? 2.f : 0.f);

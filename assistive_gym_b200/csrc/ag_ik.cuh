@@ -5,8 +5,7 @@
 // below a threshold.  SURVEY.md §8(f)1 (batched reset).  Kinematics only: reads the scene template and the body's
 // base pose, writes nothing but its outputs.
 #pragma once
-#include "ag_device.cuh"
-#include "ag_feeding.cuh"      // xorshift64s / rng_uniform
+#include "ag_task.cuh"        // xorshift64s / rng_uniform
 
 #define AG_IK_MAXCHAIN 32      // links on the path base -> end effector
 #define AG_IK_MAXJ 8           // joints solved for

@@ -11,6 +11,7 @@
 #include "../../include/agphys.h"
 #include "ag_device.cuh"
 #include "ag_solver.cuh"
+#include "ag_readback.cuh"
 #include "ag_feeding.cuh"
 #include "ag_bathing.cuh"
 #include "ag_ik.cuh"
