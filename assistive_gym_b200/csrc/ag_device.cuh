@@ -580,15 +580,15 @@ AG_HD SVf sv_add(SVf a, SVf b) { SVf r; r.a = a.a + b.a; r.l = a.l + b.l; return
 AG_HD SVf sv_scale(SVf a, float s) { SVf r; r.a = a.a * s; r.l = a.l * s; return r; }
 AG_HD float sv_dot(SVf m, SVf f) { return dot(m.a, f.a) + dot(m.l, f.l); }
 
-// One lane per env: free bodies (gravity, damping, gyroscopic) and articulated bodies (ABA + M^-1).
-// thread = (work item, env): work items 0..nf-1 are the free bodies, nf..nf+nart-1 the articulated bodies (independent of each other)
-AG_HDN inline void dyn_body(int tid, const SimDev& S, const KP&) {
+// K5: one lane per (body, env): free bodies (gravity, damping, gyroscopic) and articulated bodies (ABA + M^-1), all
+// independent of each other.
+// thread = (free body f, env), tid = f * N + e
+AG_HDN inline void dyn_free_body(int tid, const SimDev& S) {
   const int N = S.N;
-  const int e = tid % N, work = tid / N;
+  const int e = tid % N;
   const float dt = S.dt, vmax = S.vmax, kl = S.lin_damp, ka = S.ang_damp;
-  // ---- free rigid bodies
-  if (work < S.nf) {
-    const int f = work;
+  {
+    const int f = tid / N;
     int b = AG_LDG(S.free_body + f);
     int l0 = AG_LDG(S.body_link0 + b);
     q4 q = ld4(S.lquat, l0, N, e);
@@ -617,17 +617,33 @@ AG_HDN inline void dyn_body(int tid, const SimDev& S, const KP&) {
     st3(S.base_lin, b, N, e, v); st3(S.base_ang, b, N, e, w);
     S.fIinv[ib] = Iinv.xx; S.fIinv[ib + N] = Iinv.yy; S.fIinv[ib + 2 * (size_t)N] = Iinv.zz;
     S.fIinv[ib + 3 * (size_t)N] = Iinv.xy; S.fIinv[ib + 4 * (size_t)N] = Iinv.xz; S.fIinv[ib + 5 * (size_t)N] = Iinv.yz;
-    return;
   }
-  // ---- articulated bodies
+}
+// Per-dof arrays of dyn_art_body: DYN_DOF_WORDS 4-byte words per dof of `cap` (the largest articulation), one word more
+// per thread so that the stride between threads is odd and a warp's accesses to the same field hit 32 distinct banks.
+#define DYN_DOF_WORDS 56      // AI 21, SVf x 4 (pA U c vel) 24, f3 x 2 (ax rr) 6, Dinv u qd 3, par typ 2
+AG_HD int dyn_scratch_words(int cap) { return DYN_DOF_WORDS * cap + 1; }
+// thread = (articulated body a, env), tid = a * N + e; `w` holds dyn_scratch_words(cap) words, cap >= the body's dofs
+AG_HDN inline void dyn_art_body(int tid, const SimDev& S, float* w, int cap) {
+  const int N = S.N;
+  const int e = tid % N;
+  const float dt = S.dt, vmax = S.vmax, kl = S.lin_damp, ka = S.ang_damp;
   {
-    const int a = work - S.nf;
+    const int a = tid / N;
     int b = AG_LDG(S.art_body + a), d0 = AG_LDG(S.art_dl0 + a), nd = AG_LDG(S.art_nd + a);
     bool active = S.body_mode[(size_t)b * N + e] == 1;
-    AI IA[AG_MAXND]; SVf pA[AG_MAXND], U[AG_MAXND], c[AG_MAXND], vel[AG_MAXND];
-    f3 ax[AG_MAXND], rr[AG_MAXND];
-    float Dinv[AG_MAXND], u[AG_MAXND], qd[AG_MAXND];
-    int par[AG_MAXND], typ[AG_MAXND];
+    AI* IA = (AI*)w; w += 21 * cap;
+    SVf* pA = (SVf*)w; w += 6 * cap;
+    SVf* U = (SVf*)w; w += 6 * cap;
+    SVf* c = (SVf*)w; w += 6 * cap;
+    SVf* vel = (SVf*)w; w += 6 * cap;
+    f3* ax = (f3*)w; w += 3 * cap;
+    f3* rr = (f3*)w; w += 3 * cap;
+    float* Dinv = w; w += cap;
+    float* u = w; w += cap;
+    float* qd = w; w += cap;
+    int* par = (int*)w; w += cap;
+    int* typ = (int*)w;
     f3 g = tv3(S.body_gravity, b);
     int l0 = AG_LDG(S.body_link0 + b);
     f3 obase = ld3(S.lpos, l0, N, e);
@@ -692,8 +708,8 @@ AG_HDN inline void dyn_body(int tid, const SimDev& S, const KP&) {
         pA[par[i]].l = pA[par[i]].l + pa.l;
       }
     }
-    // pass 3: accelerations, root to leaf
-    SVf acc[AG_MAXND];
+    // pass 3: accelerations, root to leaf (in vel's words: velocities are not read after pass 1)
+    SVf* acc = vel;
     for (int i = 0; i < nd; i++) {
       SVf ap; if (par[i] >= 0) ap = acc[par[i]]; else { ap.l = -g; }
       SVf a1; a1.a = ap.a + c[i].a; a1.l = ap.l + cross(ap.a, rr[i]) + c[i].l;
@@ -703,9 +719,10 @@ AG_HDN inline void dyn_body(int tid, const SimDev& S, const KP&) {
       float nq = clampf(qd[i] + dt * qdd, -vmax, vmax);
       if (active) st1(S.jqd, AG_LDG(S.dl_link + d0 + i), N, e, nq);
     }
-    // M^-1 by unit joint impulses through the cached articulated inertias
+    // M^-1 by unit joint impulses through the cached articulated inertias; p, uu and aa reuse the words of pA, qd and
+    // acc, which are not read after passes 2 and 3
+    SVf* p = pA; float* uu = qd; SVf* aa = acc;
     for (int j = 0; j < nd; j++) {
-      SVf p[AG_MAXND]; float uu[AG_MAXND];
       for (int i = 0; i < nd; i++) { p[i] = SVf(); }
       for (int i = nd - 1; i >= 0; i--) {
         SVf Sx; if (typ[i] == 1) Sx.a = ax[i]; else Sx.l = ax[i];
@@ -716,7 +733,6 @@ AG_HDN inline void dyn_body(int tid, const SimDev& S, const KP&) {
           p[par[i]].l = p[par[i]].l + pa.l;
         }
       }
-      SVf aa[AG_MAXND];
       for (int i = 0; i < nd; i++) {
         SVf ap; if (par[i] >= 0) ap = aa[par[i]];
         SVf a1; a1.a = ap.a; a1.l = ap.l + cross(ap.a, rr[i]);

@@ -106,10 +106,12 @@ AG_HD RsShape rs_shape(const SimDev& S, int refA, int refB) {
   side_dims(S, refA, h.offA, h.nA); side_dims(S, refB, h.offB, h.nB);
   h.merged = h.nA > 0 && h.nB > 0 && h.offA == h.offB;
   const int null = rs_null(S);
-  h.nv = 0; h.sl[0] = h.sl[1] = h.sl[2] = h.sl[3] = null;
-  if (h.nA > 0) { h.sl[h.nv++] = h.offA; if (h.nA > 8) h.sl[h.nv++] = h.offA + 8; }
-  h.slotB = h.merged ? 0 : h.nv;
-  if (h.nB > 0 && !h.merged) { h.sl[h.nv++] = h.offB; if (h.nB > 8) h.sl[h.nv++] = h.offB + 8; }
+  // blocks of A, then of B; every index into sl is a constant, so the shape stays in registers
+  const int na = h.nA > 0 ? (h.nA > 8 ? 2 : 1) : 0, nb = (h.nB > 0 && !h.merged) ? (h.nB > 8 ? 2 : 1) : 0;
+#pragma unroll
+  for (int k = 0; k < 4; k++) h.sl[k] = k < na ? h.offA + 8 * k : (k < na + nb ? h.offB + 8 * (k - na) : null);
+  h.nv = na + nb;
+  h.slotB = h.merged ? 0 : na;
   return h;
 }
 AG_HD int rs_shape_key(const RsShape& h) { return h.nv == 0 ? -1 : (h.sl[0] | (h.merged ? 0x8000 : 0) | ((h.nB > 0 && !h.merged ? h.offB + 1 : 0) << 16)); }
@@ -141,21 +143,30 @@ AG_HDN inline void emit_side(const SimDev& S, int e, int ref, f3 p, f3 lin, f3 a
     float M[6] = {lin.x * invm, lin.y * invm, lin.z * invm, it.x, it.y, it.z};
     for (int i = 0; i < 6; i++) { float* d = rs_entry(rec, slot0, i, row); d[0] = J[i]; d[1] = M[i]; }
   } else if (kind == 2) {
+    // J lives in registers: every index into it is a constant of the unrolled loops.  A dof's parent precedes it
+    // (dyn_body's leaf-to-root pass relies on the same order), so one downward sweep meets the whole chain from idx.
     float J[AG_MAXND];
     int a = AG_LDG(S.dl_art + idx), d0 = AG_LDG(S.art_dl0 + a), nd = AG_LDG(S.art_nd + a);
-    for (int i = 0; i < nd; i++) J[i] = 0.f;
     int j = idx;
-    while (j >= 0) {
-      f3 axw = ld3(S.jax, j, N, e), o = ld3(S.jor, j, N, e);
-      J[j - d0] = (AG_LDG(S.dl_type + j) == 1) ? (dot(lin, cross(axw, p - o)) + dot(ang, axw)) : dot(lin, axw);
-      j = AG_LDG(S.dl_parent + j);
+#pragma unroll
+    for (int i = AG_MAXND - 1; i >= 0; i--) {
+      J[i] = 0.f;
+      if (i < nd && d0 + i == j) {
+        f3 axw = ld3(S.jax, j, N, e), o = ld3(S.jor, j, N, e);
+        J[i] = (AG_LDG(S.dl_type + j) == 1) ? (dot(lin, cross(axw, p - o)) + dot(ang, axw)) : dot(lin, axw);
+        j = AG_LDG(S.dl_parent + j);
+      }
     }
     for (int i = 0; i < nd; i++) {
-      float m = 0.f;
-      for (int k = 0; k < nd; k++) m += S.Minv[((size_t)(d0 + i) * S.ND + (d0 + k)) * N + e] * J[k];
+      float m = 0.f, Ji = 0.f;
+#pragma unroll
+      for (int k = 0; k < AG_MAXND; k++) {
+        if (k < nd) m += S.Minv[((size_t)(d0 + i) * S.ND + (d0 + k)) * N + e] * J[k];
+        if (k == i) Ji = J[k];
+      }
       float* d = rs_entry(rec, slot0, i, row);
-      if (acc) { d[0] += J[i]; d[1] += m; } else { d[0] = J[i]; d[1] = m; }
-      rel += J[i] * ld1(S.jqd, AG_LDG(S.dl_link + d0 + i), N, e);
+      if (acc) { d[0] += Ji; d[1] += m; } else { d[0] = Ji; d[1] = m; }
+      rel += Ji * ld1(S.jqd, AG_LDG(S.dl_link + d0 + i), N, e);
     }
   }
 }
@@ -361,13 +372,14 @@ AG_HD void rs_finish_box(const SimDev& S, float* rec, int nv, int row, int li, f
   else rs_null_row(rec, nv, row);
 }
 
-// K6b, rows part: thread = (dof / fixed-constraint row r, env): the thread of a record's FIRST row writes the whole record
-AG_HDN inline void drow_body(int r, int e, const SimDev& S) {
+// K6b, rows part: thread = (dof / fixed-constraint row r, env): the thread of a record's FIRST row builds the whole record
+// in `rec` (see crows_record)
+AG_HDN inline int drow_body(int r, int e, const SimDev& S, float* rec, float*& dst) {
   const int N = S.N;
   const float dt = S.dt;
   int info = S.row_off[(size_t)r * N + e];
-  if (info < 0 || (info & 1)) return;
-  float* rec = S.rs_data + (size_t)e * S.rs_cap + (size_t)(info >> 2) * RS_UNIT;
+  if (info < 0 || (info & 1)) return 0;
+  dst = S.rs_data + (size_t)e * S.rs_cap + (size_t)(info >> 2) * RS_UNIT;
   const int r2 = (info & 2) ? S.row_pair[(size_t)r * N + e] : -1;
   if (r < 3 * S.ND) {
     int d = r % S.ND;
@@ -376,7 +388,9 @@ AG_HDN inline void drow_body(int r, int e, const SimDev& S) {
     rs_header(S, rec, h, RM_BOX);
     rs_zero_blocks(rec, h.nv);
     int dd[2] = {d, 0}; float sg[2] = {1.f, 1.f};
-    for (int row = 0; row < (r2 >= 0 ? 2 : 1); row++) {
+#pragma unroll
+    for (int row = 0; row < 2; row++) {
+      if (row == 1 && r2 < 0) break;
       int rr = row == 0 ? r : r2;
       int kind = rr / S.ND; dd[row] = rr % S.ND;
       DofRow R;
@@ -390,12 +404,12 @@ AG_HDN inline void drow_body(int r, int e, const SimDev& S) {
       rs_set_row(S, rec, row, rr, R.rhs, R.dinv, R.lo, R.hi);
     }
     if (r2 >= 0) rec[5] = sg[0] * sg[1] * S.Minv[((size_t)dd[1] * S.ND + dd[0]) * N + e];
-    return;
+    return rs_rec_floats(h.nv);
   }
   // fixed constraint c, rows i and i + 1: 3 translation + 3 rotation rows
   int c = (r - 3 * S.ND) / 6, i0 = (r - 3 * S.ND) % 6;
   int refA, refB; bool sw;
-  if (!con_sides(S, e, c, refA, refB, sw)) return;
+  if (!con_sides(S, e, c, refA, refB, sw)) return 0;
   RsShape h = rs_shape(S, refA, refB);
   rs_header(S, rec, h, RM_BOX);
   rs_zero_blocks(rec, h.nv);
@@ -422,10 +436,10 @@ AG_HDN inline void drow_body(int r, int e, const SimDev& S) {
     rs_finish_box(S, rec, h.nv, row, r + row, -err * S.erp / dt - rel, -maxi, maxi);
   }
   if (r2 >= 0) rec[5] = rs_row_w21(rec, h.nv);
+  return rs_rec_floats(h.nv);
 }
 
-// ---- K6b fast path: records whose sides are free bodies (or static): both rows are built in registers and the record
-// goes out as 16-byte stores (header: 4, each lane block: 8) instead of ~90 scattered 4-byte stores and read-backs.
+// ---- K6b fast path: records whose sides are free bodies (or static): both rows are built in registers.
 struct FreeSide { float J[6], M[6], rel; };
 AG_HD FreeSide free_side_zero() { FreeSide r; for (int i = 0; i < 6; i++) { r.J[i] = 0.f; r.M[i] = 0.f; } r.rel = 0.f; return r; }
 // unit force `lin` at world point p on free body `idx` (side reference kind 1); anything else: zeros
@@ -476,26 +490,29 @@ AG_HD void rs_head_store(float* rec, const RsHead& H) {
 }
 
 // K6b: thread = (row, env): rows [0, maxc) are the sorted contacts, rows [maxc, maxc + 3 ND + ngr) the dof and
-// fixed-constraint rows.  The thread of contact s writes the normal record that STARTS at s (one or two rows) and the
-// friction record of s.
-AG_HDN inline void crows_body(int tid, const SimDev& S, const KP&) {
+// fixed-constraint rows.  The thread of contact s writes the normal record that STARTS at s (one or two rows), part 0,
+// and the friction record of s, part 1.  A part is built whole in `rec` (RS_MAXREC floats, 16-byte aligned, private to
+// the thread); the return value is its length in floats (0: nothing to write) and `dst` its place in the stream.  The
+// caller copies it there (k_crows: a warp stores its lanes' records as consecutive 16-byte pieces).
+AG_HDN inline int crows_record(int tid, const SimDev& S, int part, float* rec, float*& dst) {
   const int N = S.N;
   int e = tid % N, slot = tid / N;
-  if (slot >= S.maxc) { drow_body(slot - S.maxc, e, S); return; }
+  if (slot >= S.maxc) return part == 0 ? drow_body(slot - S.maxc, e, S, rec, dst) : 0;
   int cnt = S.c_count[e]; if (cnt > S.maxc) cnt = S.maxc;
-  if (slot >= cnt) return;
-  for (int d = 0; d < 3; d++) cf_st(S.s_data, slot, CF_LAM_N + d, N, e, 0.f);
+  if (slot >= cnt) return 0;
+  if (part == 0) for (int d = 0; d < 3; d++) cf_st(S.s_data, slot, CF_LAM_N + d, N, e, 0.f);
   size_t rb = (size_t)slot * 4 * N + e;
   const int refA = S.s_ref[rb], refB0 = S.s_ref[rb + N], info = S.s_ref[rb + 2 * (size_t)N], of = S.s_ref[rb + 3 * (size_t)N];
-  if (info < 0) return;
+  if (info < 0) return 0;
   const int refB = refB0 & ~(1 << 30);
   const RsShape h = rs_shape(S, refA, refB);
   float* rs = S.rs_data + (size_t)e * S.rs_cap;
   const float dt = S.dt;
   const int lam0 = 3 * S.ND + S.ngr;
   const bool fast = (refA & 3) == 1 && (refB & 3) != 2;      // sides: a free body and (nothing | a free body)
-  if (!(info & 1)) {
-    float* rec = rs + (size_t)(info >> 2) * RS_UNIT;
+  if (part == 0) {
+    if (info & 1) return 0;
+    dst = rs + (size_t)(info >> 2) * RS_UNIT;
     const int nrow = (info & 2) ? 2 : 1;
     if (fast) {
       RsHead H = rs_head(S, h, RM_BOX);
@@ -549,9 +566,10 @@ AG_HDN inline void crows_body(int tid, const SimDev& S, const KP&) {
       }
       if (nrow == 2) rec[5] = rs_row_w21(rec, h.nv);
     }
+    return rs_rec_floats(h.nv);
   }
   if (of >= 0) {
-    float* rec = rs + (size_t)of * RS_UNIT;
+    dst = rs + (size_t)of * RS_UNIT;
     f3 pa(cf_ld(S.s_data, slot, CF_PAX, N, e), cf_ld(S.s_data, slot, CF_PAY, N, e), cf_ld(S.s_data, slot, CF_PAZ, N, e));
     f3 pb(cf_ld(S.s_data, slot, CF_PBX, N, e), cf_ld(S.s_data, slot, CF_PBY, N, e), cf_ld(S.s_data, slot, CF_PBZ, N, e));
     f3 n(cf_ld(S.s_data, slot, CF_NX, N, e), cf_ld(S.s_data, slot, CF_NY, N, e), cf_ld(S.s_data, slot, CF_NZ, N, e));
@@ -591,7 +609,9 @@ AG_HDN inline void crows_body(int tid, const SimDev& S, const KP&) {
       }
       rec[4] = i2f_bits(rs_enc_lam(S, lam0 + 3 * slot)); rec[6] = mu;
     }
+    return rs_rec_floats(h.nv);
   }
+  return 0;
 }
 
 // ------------------------------------------------------------------ K6c: heaviest-first env order for K7

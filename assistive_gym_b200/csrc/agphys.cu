@@ -61,9 +61,63 @@ AG_KERNEL(k_pairs, pairs_body)
 AG_KERNEL(k_csort, csort_body)
 AG_KERNEL_B(k_narrow, narrow_body, 3)
 AG_KERNEL(k_sort, sort_body)
-AG_KERNEL(k_dyn, dyn_body)
+// k_dyn: a CTA is two warps.  Warp 0 runs DYN_T articulated bodies, each lane with its per-dof arrays in its own slice of
+// shared memory (p.i2 = dyn_scratch_words words); warp 1 steps free bodies, grid-stride over all of them, so that their
+// lanes run beside the long ABA chains instead of taking CTA slots of their own.  p.i0 = nart * N, p.i1 = nf * N.
+#define DYN_T 32
+#ifndef AG_CPU_EMU
+__global__ void __launch_bounds__(2 * DYN_T) k_dyn(SimDev S, KP p) {
+  extern __shared__ float dyn_smem[];
+  if (threadIdx.x < DYN_T) {
+    const int t = blockIdx.x * DYN_T + threadIdx.x;
+    if (t < p.i0) dyn_art_body(t, S, dyn_smem + threadIdx.x * p.i2, p.i3);
+  } else {
+    for (int t = blockIdx.x * DYN_T + threadIdx.x - DYN_T; t < p.i1; t += gridDim.x * DYN_T) dyn_free_body(t, S);
+  }
+}
+#else
+static void k_dyn(SimDev S, KP p) {
+  std::vector<float> w((size_t)p.i2);
+  for (int t = 0; t < p.i1; t++) dyn_free_body(t, S);
+  for (int t = 0; t < p.i0; t++) dyn_art_body(t, S, w.data(), p.i3);
+}
+#endif
 AG_KERNEL(k_rows, rows_body)
-AG_KERNEL(k_crows, crows_body)
+// k_crows: each thread builds its records one at a time in its own slice of shared memory; then the warp stores every
+// lane's record in turn, lane l taking the record's 16-byte piece l (and l + 32), so one store instruction writes 512
+// contiguous bytes of one env's stream instead of 16 bytes (or 4) in each of 32 envs' streams.
+#define CROWS_T 64
+#define CROWS_STRIDE (RS_MAXREC + 4)    // 37 16-byte units (odd): eight lanes' 16-byte accesses at one offset hit distinct banks
+#ifndef AG_CPU_EMU
+__global__ void __launch_bounds__(CROWS_T) k_crows(SimDev S, KP p) {
+  __shared__ __align__(16) float stage[CROWS_T * CROWS_STRIDE];
+  const int tid = blockIdx.x * blockDim.x + threadIdx.x, lane = threadIdx.x & 31;
+  const float* wstage = stage + (threadIdx.x - lane) * CROWS_STRIDE;
+  for (int part = 0; part < 2; part++) {
+    float* dst = nullptr;
+    const int nf = tid < p.n ? crows_record(tid, S, part, stage + threadIdx.x * CROWS_STRIDE, dst) : 0;
+    __syncwarp();
+    unsigned todo = __ballot_sync(~0u, nf > 0);
+    while (todo) {
+      const int j = __ffs(todo) - 1; todo &= todo - 1;
+      const int n = __shfl_sync(~0u, nf, j);
+      float* d = (float*)__shfl_sync(~0u, (unsigned long long)dst, j);
+      for (int k = 4 * lane; k < n; k += 128) stv4(d + k, ldv4(wstage + j * CROWS_STRIDE + k));
+    }
+    __syncwarp();
+  }
+}
+#else
+static void k_crows(SimDev S, KP p) {
+  alignas(16) float rec[RS_MAXREC];
+  for (int tid = 0; tid < p.n; tid++)
+    for (int part = 0; part < 2; part++) {
+      float* dst = nullptr;
+      const int nf = crows_record(tid, S, part, rec, dst);
+      std::copy(rec, rec + nf, dst);
+    }
+}
+#endif
 // k_pgs: one warp per CTA = RS_CTA_ENVS (8) envs, four lanes each; per-env shared memory = velocity deltas + impulses +
 // a 4 KB row-stream ring (TMA bulk copy for the first tile, cp.async refill; see ag_solver.cuh).
 // k_order: heaviest-first env order for k_pgs (64-bucket counting sort, one CTA).
@@ -194,6 +248,7 @@ struct AgSim {
   // host copies of template info needed by the API
   std::vector<int> body_link0, body_nlinks, body_kind, link_body;
   int nl, nb;
+  int dyn_cap;                         // dofs of the largest articulated body (k_dyn's per-thread scratch)
   // staging
   float* d_stage; size_t stage_floats;
   std::vector<float> h_stage;
@@ -475,6 +530,8 @@ AgSim* ag_create(const AgSceneDesc* d, const AgConfig* cfg, int n_envs, int devi
   }
   S.nf = (int)free_body.size(); S.nart = (int)art_body.size(); S.ND = (int)dl_link.size(); S.nparts = (int)pt_mass.size();
   for (int nd_a : art_nd) if (nd_a > AG_MAXND) { g_err = "too many DoFs in one articulated body (AG_MAXND)"; ag_destroy(s); return nullptr; }
+  s->dyn_cap = 1;
+  for (int nd_a : art_nd) s->dyn_cap = std::max(s->dyn_cap, nd_a);
   if (S.ND > 32) { g_err = "too many articulated DoFs per env (32)"; ag_destroy(s); return nullptr; }
   s->body_kind = body_kind;
   // movable lists
@@ -598,6 +655,8 @@ AgSim* ag_create(const AgSceneDesc* d, const AgConfig* cfg, int n_envs, int devi
     size_t smem = (size_t)rs_cta_floats(S) * sizeof(float);
     if (smem > 227 * 1024) { g_err = "PGS shared-memory footprint exceeds 227 KB per CTA: lower max_contacts"; ag_destroy(s); return nullptr; }
     if (cudaFuncSetAttribute(k_pgs, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { g_err = "cudaFuncSetAttribute(k_pgs) failed"; ag_destroy(s); return nullptr; }
+    const int dyn_smem = DYN_T * dyn_scratch_words(AG_MAXND) * (int)sizeof(float);     // 112 KB: the largest any scene asks for
+    if (cudaFuncSetAttribute(k_dyn, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn_smem) != cudaSuccess) { g_err = "cudaFuncSetAttribute(k_dyn) failed"; ag_destroy(s); return nullptr; }
   }
 #endif
   // defaults: friction from the template, all bodies active, identity quaternions
@@ -839,10 +898,32 @@ static void substep(AgSim* s) {
   LAUNCH(s, k_csort, (size_t)S.maxcand * N, z);
   LAUNCH(s, k_narrow, (size_t)S.maxcand * N, z);
   LAUNCH(s, k_sort, (size_t)S.maxraw * N, z);
-  LAUNCH(s, k_dyn, (size_t)(S.nf + S.nart) * N, z);
-  LAUNCH(s, k_rows, N, z);
-  LAUNCH(s, k_crows, (size_t)(S.maxc + 3 * S.ND + S.ngr) * N, z);
+  {
+    KP d = z; d.i0 = S.nart * N; d.i1 = S.nf * N; d.i3 = s->dyn_cap; d.i2 = dyn_scratch_words(d.i3);
 #ifndef AG_CPU_EMU
+    // enough CTAs for every articulated body, and at least one per eight free bodies' lanes
+    int nblk = std::max((d.i0 + DYN_T - 1) / DYN_T, (d.i1 + 8 * DYN_T - 1) / (8 * DYN_T));
+    if (nblk > 0) {
+      int ps = s->profiling ? prof_slot(s, "k_dyn") : -1;
+      if (ps >= 0) prof_mark(s, ps, true);
+      k_dyn<<<nblk, 2 * DYN_T, (size_t)(d.i0 > 0 ? DYN_T * d.i2 : 0) * sizeof(float), s->stream>>>(S, d);
+      if (ps >= 0) prof_mark(s, ps, false);
+      s->launches++;
+    }
+#else
+    LAUNCH(s, k_dyn, (size_t)(S.nf + S.nart) * N, d);
+#endif
+  }
+  LAUNCH(s, k_rows, N, z);
+#ifndef AG_CPU_EMU
+  {
+    KP kp = z; kp.n = (S.maxc + 3 * S.ND + S.ngr) * N;
+    int ps = s->profiling ? prof_slot(s, "k_crows") : -1;
+    if (ps >= 0) prof_mark(s, ps, true);
+    k_crows<<<(kp.n + CROWS_T - 1) / CROWS_T, CROWS_T, 0, s->stream>>>(S, kp);
+    if (ps >= 0) prof_mark(s, ps, false);
+    s->launches++;
+  }
   {
     int ps = s->profiling ? prof_slot(s, "k_order") : -1;
     if (ps >= 0) prof_mark(s, ps, true);
@@ -857,6 +938,7 @@ static void substep(AgSim* s) {
     s->launches += 2;
   }
 #else
+  LAUNCH(s, k_crows, (size_t)(S.maxc + 3 * S.ND + S.ngr) * N, z);
   k_order(S, z);
   LAUNCH(s, k_pgs, N, z);
   LAUNCH(s, k_integrate, N, z);                      // (fused into k_pgs on the device)
