@@ -24,20 +24,19 @@ once per stepSimulation (env.py:226-231), as `k_coop_limits` does.
 """
 import numpy as np
 
-from . import capi
+from . import capi, toc
 from .cloth import ClothModel
 from .feeding_batch import coop_params, pack_mlp
 from .human_model import create_human
-from .kinematics import BodyKinematics, q_axis, q_from_rpy, q_mul, q_rot
-from .toc import jlwki, position_robot_toc  # noqa: F401
+from .kinematics import q_axis, q_from_rpy, q_mul, q_rot
+from .toc import TocPlacement, jlwki, position_robot_toc  # noqa: F401
 from .scene import SceneBuilder, quat_from_rpy
 
 MOTOR_POSITION = 1
 
-PR2 = dict(arm=[64, 65, 66, 68, 69, 71, 72], ee=76, gripper=[79, 80, 81, 82], gripper_pos=[0.0] * 4,
-           right_arm=[42, 43, 44, 46, 47, 49, 50], right_preset=[-1.75, 1.25, -1.5, -0.5, -1, 0, -1],
-           left_preset=[1.75, 1.25, 1.5, -0.5, 1, 0, 1],
-           toc_base_pos_offset=[1.7, 0.7, 0], ee_orient_rpy=[0, 0, np.pi], ee_orient_shoulder_rpy=[0, 0, np.pi * 3 / 2.0])
+PR2 = dict(toc.PR2_LEFT, gripper_pos=[0.0] * 4, right_arm=toc.PR2_RIGHT['arm'], right_preset=toc.PR2_RIGHT['default_q'],
+           left_preset=toc.PR2_LEFT['default_q'], toc_base_pos_offset=[1.7, 0.7, 0], ee_orient_rpy=[0, 0, np.pi],
+           ee_orient_shoulder_rpy=[0, 0, np.pi * 3 / 2.0])
 LEFT_ARM_JOINTS = list(range(10, 20))                       # human.left_arm_joints (dressing_envs.py)
 L_SHOULDER, L_ELBOW, L_WRIST = 15, 17, 19                   # human.py:26-28
 L_ARM_LIMIT_JOINTS = [13, 14, 15, 16]                       # left shoulder x, y, z and elbow: the classifier's inputs (human.py:137-140)
@@ -83,14 +82,22 @@ def sleeve_on_arm_reward(triangle1_points, triangle2_points, shoulder_pos, elbow
             np.linalg.norm(elbow_end - centre), np.linalg.norm(shoulder_end - centre), np.linalg.norm(hand_end - elbow_end), np.linalg.norm(el - sh))
 
 
-class DressingBatch:
+class DressingBatch(TocPlacement):
+    """DressingPR2-v1 / DressingPR2Human-v1.  The robot is the scene's only per-robot part: `R` and `load_robot` / `robot_links`
+    (TocPlacement) build it, `CLOTH_ROBOT_JOINTS` picks the links the gown collides with, and `_reset_robot` puts it in place;
+    dressing_robots_batch.py replaces these for Sawyer and Jaco and shares the rest."""
+    R = PR2
+    WHEELCHAIR = 'wheelchair'
+    # PR2: its left arm and gripper (everything else of PR2 stays a metre away from the gown)
+    CLOTH_ROBOT_JOINTS = range(PR2['arm'][0], 86)
+
     def __init__(self, controllable_person=False):
         self.controllable_person = bool(controllable_person)
         b = SceneBuilder()
         self.builder = b
         b.set_gravity([0, 0, -9.81])
         self.plane = b.load_urdf('plane')
-        self.wheelchair = b.load_urdf('wheelchair', base_pos=[0, 0, 0.06], fixed_base=False)
+        self.wheelchair = b.load_urdf(self.WHEELCHAIR, base_pos=[0, 0, 0.06], fixed_base=False)
         self.humans = {}
         for gender, z in (('male', 0.89), ('female', 0.86)):
             hb, info = create_human(b, gender=gender, static=True, cloth=True)       # env.py:38 cloth=('dressing' in task)
@@ -100,29 +107,21 @@ class DressingBatch:
                     b.change_dynamics(hb, j, mass=0)
             b.set_gravity([0, 0, -1], body=hb)                                        # dressing.py:181
             self.humans[gender] = hb
-        self.robot = b.load_urdf('pr2', base_pos=[-1, -1, 0], fixed_base=True, inertia_from_file=True)    # pr2.py:52
-        b.weld_joints(self.robot, set(PR2['arm']) | set(PR2['gripper']), dict(zip(PR2['right_arm'], PR2['right_preset'])))
-        b.continuous_limits_for_ik(self.robot, PR2['arm'])
+        self.load_robot(b)                                                            # PR2: pr2.py:52
         b.set_gravity([0, 0, 0], body=self.robot)                                     # dressing.py:179-180
         self.scene = b.finalize()
         sc = self.scene
-        self.gl = lambda body, link: int(sc['body_link0'][body]) + 1 + link
-        self.arm_links = [self.gl(self.robot, j) for j in PR2['arm']]
-        self.gripper_links = [self.gl(self.robot, j) for j in PR2['gripper']]
-        self.ee_link = self.gl(self.robot, PR2['ee'])
-        self.kin = BodyKinematics(sc, self.robot)
-        self.arm_lower = sc['link_lower'][self.arm_links].copy()
-        self.arm_upper = sc['link_upper'][self.arm_links].copy()
-        nolimit = sc['link_haslimit'][self.arm_links] == 0
-        self.arm_lower[nolimit], self.arm_upper[nolimit] = -1e10, 1e10
+        self.robot_links(sc)
+        self.tool = None
+        self.obstacles = (self.humans['male'], self.humans['female'], self.wheelchair)       # collision_objects of dressing.py:134
         self.human_arm_links = {g: [self.gl(hb, j) for j in LEFT_ARM_JOINTS] for g, hb in self.humans.items()}
-        # ---- cloth template and the rigid links it collides with: the person, the robot's left arm and gripper, the
-        # wheelchair and the ground (everything else of PR2 stays a metre away from the gown)
+        # ---- cloth template and the rigid links it collides with: the person, the robot's `CLOTH_ROBOT_JOINTS`, the wheelchair
+        # and the ground
         self.cloth = ClothModel.load('hospitalgown_reduced', scale=CLOTH_SCALE)
         has_col = lambda k: np.any(sc['col_link'] == k)
         links, static = [], []
         for body, is_static, rng_ in ([(self.plane, 1, None), (self.wheelchair, 1, None)] + [(hb, 0, None) for hb in self.humans.values()]
-                                      + [(self.robot, 0, range(PR2['arm'][0], 86))]):
+                                      + [(self.robot, 0, self.CLOTH_ROBOT_JOINTS)]):
             l0, nl = int(sc['body_link0'][body]), int(sc['body_nlinks'][body])
             for k in range(l0, l0 + nl):
                 if rng_ is not None and (k - l0 - 1) not in rng_:
@@ -203,12 +202,25 @@ class DressingBatch:
 
     def reset(self, sim, rng, sample=None, attempts=50, settle_steps=50, outer_iterations=3):
         n = sim.n
-        sc = self.scene
         s = sample or self.sample(n, rng)
         self.last_sample = s
+        limb = self._reset_person(sim, s)
+        base_pos, base_quat, q7, gq = self._reset_robot(sim, s, rng, limb, attempts, outer_iterations)
+        ng = len(self.gripper_links)
+        sim.set_motor(self.arm_links, MOTOR_POSITION, target=q7, kp=[0.01] * 7, kd=[1.0] * 7, max_force=[1.0] * 7)       # dressing.py:117
+        sim.set_motor(self.gripper_links, MOTOR_POSITION, target=gq, kp=[0.05] * ng, kd=[1.0] * ng, max_force=[500.0] * ng)
+        sim.forward_kinematics()
+        self.base_pos, self.base_quat = base_pos, base_quat
+        self._reset_cloth(sim, settle_steps)
+        return s
+
+    def _reset_person(self, sim, s):
+        """Floor friction; the person seated in the wheelchair, the left arm held by weak position motors (dressing.py:117-121);
+        returns the active person's left shoulder, elbow and wrist [n, 3, 3]."""
+        n = sim.n
+        sc = self.scene
         male = s['male'].astype(bool)
         sim.set_link_friction(int(sc['body_link0'][self.plane]), s['plane_friction'])
-        # ---- person seated in the wheelchair, left arm held by weak position motors (dressing.py:117-121)
         for g, hb in self.humans.items():
             links, q = self.human_pose()[g]
             qn = np.tile(q, (n, 1))
@@ -233,7 +245,12 @@ class DressingBatch:
         for g, hb in self.humans.items():
             ls = sim.get_link_states([self.gl(hb, L_SHOULDER), self.gl(hb, L_ELBOW), self.gl(hb, L_WRIST)])['pos']
             limb[male if g == 'male' else ~male] = ls[male if g == 'male' else ~male]
-        # ---- robot base pose and start joint angles (dressing.py:129-134)
+        return limb
+
+    def _reset_robot(self, sim, s, rng, limb, attempts, outer_iterations):
+        """PR2's base pose and start joint angles (dressing.py:129-134); returns base position, base orientation, arm angles and the
+        gripper's motor targets."""
+        n = sim.n
         replay = 'base_pos' in s
         tq = np.tile(q_from_rpy(PR2['ee_orient_rpy']), (n, 1)); tqs = np.tile(q_from_rpy(PR2['ee_orient_shoulder_rpy']), (n, 1))
         target = np.array([0.45, -0.3, 1.0]) + s['ee_offset']
@@ -253,10 +270,7 @@ class DressingBatch:
                 sim.set_base_pose(self.robot, base_pos, base_quat)
                 sim.set_joint_state(self.arm_links, q=q7, qd=np.zeros_like(q7))
                 sim.forward_kinematics()
-                hit = np.zeros(n, dtype=bool)
-                for ob in (self.humans['male'], self.humans['female'], self.wheelchair):
-                    hit |= sim.closest_points(self.robot, ob, 0.0, max_pts=1)[1] > 0
-                todo = hit
+                todo = self.colliding(sim)
                 if not todo.any():
                     break
             self.unresolved = int(todo.sum())
@@ -264,11 +278,10 @@ class DressingBatch:
             s.update(base_pos=base_pos.copy(), base_quat=base_quat.copy(), q7=q7.copy(), goals_reached=reached.copy())
         sim.set_base_pose(self.robot, base_pos, base_quat)
         sim.set_joint_state(self.arm_links, q=q7, qd=np.zeros_like(q7))
-        sim.set_motor(self.arm_links, MOTOR_POSITION, target=q7, kp=[0.01] * 7, kd=[1.0] * 7, max_force=[1.0] * 7)       # dressing.py:117
-        sim.set_motor(self.gripper_links, MOTOR_POSITION, target=gq, kp=[0.05] * 4, kd=[1.0] * 4, max_force=[500.0] * 4)
-        sim.forward_kinematics()
-        self.base_pos, self.base_quat = base_pos, base_quat
-        # ---- cloth: placed relative to the end effector, four nodes anchored to it, settled at half gravity (dressing.py:139-193)
+        return base_pos, base_quat, q7, gq
+
+    def _reset_cloth(self, sim, settle_steps):
+        """The gown placed relative to the end effector, four nodes anchored to it, settled at half gravity (dressing.py:139-193)."""
         start_ee = sim.get_link_states([self.ee_link])['pos'][:, 0].astype(np.float64)
         self.start_ee_pos = start_ee
         x0 = self.x_zero[None] + (start_ee - CLOTH_ORIG_POS)[:, None, :]
@@ -284,7 +297,6 @@ class DressingBatch:
         # first substeps of the settle a few per cent of the envs hold more cloth contacts than the 1 024-contact budget; reported
         # separately from the steady-state flag, which the caller reads after its own steps
         self.settle_overflow = int(sim.overflow_count()) if hasattr(sim, 'overflow_count') else 0
-        return s
 
     def person_limits(self, links):
         """Template limits of the person's joints as the per-call Agent sees them (an unlimited joint is +-1e10, agent.py)."""

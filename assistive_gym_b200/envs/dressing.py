@@ -4,7 +4,9 @@
 cloth's anchor follows the end effector) -> sleeve-on-arm reward, cloth forces, obs[24] / reward / done.  `_get_obs` (used
 by `reset`) reads the same quantities through the per-call Agent API.
 
-With a controllable person (co-optimisation, `DressingPR2Human-v1`) `step` takes {'robot': a7, 'human': a10} and goes through the
+The robot is PR2 or Sawyer placed by TOC, or the wheelchair-mounted Jaco (`dressing_batch_for`).
+
+With a controllable person (co-optimisation, `Dressing{PR2,Sawyer,Jaco}Human-v1`) `step` takes {'robot': a7, 'human': a10} and goes through the
 per-call path (`step_reference_api`): `take_step` drives the person's left arm and, after every stepSimulation, keeps it inside its
 (per-env scaled) limits and the realistic joint limits (human.py:134-152), then moves the gown's anchor to the end effector
 (`update_targets`); the observation, the sleeve-on-arm reward and the cloth forces are computed on the host.  `step_fused` runs
@@ -17,12 +19,22 @@ from ..sim import BatchSim
 from .env import AssistiveEnv
 
 
+def dressing_batch_for(robot, controllable_person=False):
+    """The batched scene of `robot`'s Dressing id: PR2 or Sawyer placed by TOC, or the wheelchair-mounted Jaco."""
+    from ..dressing_robots_batch import DressingJacoBatch, DressingSawyerBatch
+    from .agents.robot import PR2, Jaco, Sawyer
+    for cls, batch in ((PR2, DressingBatch), (Sawyer, DressingSawyerBatch), (Jaco, DressingJacoBatch)):
+        if type(robot) is cls:
+            return batch(controllable_person=controllable_person)
+    raise KeyError('Dressing is not built for %s' % type(robot).__name__)
+
+
 class DressingEnv(AssistiveEnv):
     def __init__(self, robot, human, n_envs=1, device=0, seed=1001, config=None, toc_attempts=50):
         super().__init__(robot=robot, human=human, task='dressing', n_envs=n_envs, device=device, seed=seed,
                          obs_robot_len=(17 + len(robot.controllable_joint_indices) - (len(robot.wheel_joint_indices) if robot.mobile else 0)),
                          obs_human_len=(18 + len(human.controllable_joint_indices)))
-        self._db = DressingBatch(controllable_person=human.controllable)
+        self._db = dressing_batch_for(robot, controllable_person=human.controllable)
         self._cfg = config or DressingBatch.config()                       # numSubSteps = 8 (dressing.py:184)
         self._toc_attempts = toc_attempts
         self._sim_lib = None

@@ -96,9 +96,9 @@ def position_robot_toc(sim, rng, robot_body, arm_links, ee_link, kin, arm_local,
 class TocPlacement:
     """`init_robot_pose`'s TOC branch (env.py:276-310) for a batched scene whose robot is not wheelchair-mounted: a TOC search,
     then a collision check of robot and tool against `obstacles`, re-searching only the colliding envs for up to `max_iterations`
-    rounds.  The scene class provides `R` (the robot's task constants), `robot`, `tool`, `kin`, `arm_links`, `gripper_links`,
-    `ee_link`, `arm_lower`, `arm_upper`, `tool_pos_offset`, `tool_quat_offset` and `obstacles`; `load_robot` and `robot_links`
-    set the robot's part of these."""
+    rounds.  A wheelchair-mounted robot (DressingJaco) uses only the robot loading, `place_robot` and `colliding`.  The scene class
+    provides `R` (the robot's task constants), `robot`, `tool` (None for a task without one: Dressing), `kin`, `arm_links`, `gripper_links`, `ee_link`, `arm_lower`, `arm_upper`, `tool_pos_offset`, `tool_quat_offset`
+    and `obstacles`; `load_robot` and `robot_links` set the robot's part of these."""
 
     def load_robot(self, b):
         """Load the robot of `R` into the scene builder `b` and weld every joint but the arm and the gripper."""
@@ -132,7 +132,7 @@ class TocPlacement:
 
     def place_robot(self, sim, base_pos, base_quat, q7):
         """Robot base, arm, open gripper and the tool at the tool joint's COM frame composed with the offsets (tool.py:49-54);
-        returns the tool's position."""
+        returns the tool's position (None without a tool)."""
         n, R = sim.n, self.R
         sim.set_base_pose(self.robot, base_pos, base_quat)
         sim.set_base_velocity(self.robot, np.zeros((n, 3)), np.zeros((n, 3)))
@@ -142,6 +142,9 @@ class TocPlacement:
         sc = self.scene
         gq = np.clip(gq, sc['link_lower'][self.gripper_links], sc['link_upper'][self.gripper_links])
         sim.set_joint_state(self.gripper_links, q=gq, qd=np.zeros_like(gq))
+        if self.tool is None:
+            sim.forward_kinematics()
+            return None
         qfull = np.zeros((n, self.kin.nl))
         qfull[:, np.array(R['arm']) + 1] = q7
         qfull[:, np.array(R['gripper']) + 1] = gq
@@ -159,11 +162,12 @@ class TocPlacement:
         hit = np.zeros(sim.n, dtype=bool)
         for ob in self.obstacles:
             hit |= sim.closest_points(self.robot, ob, 0.0, max_pts=1)[1] > 0
-            hit |= sim.closest_points(self.tool, ob, 0.0, max_pts=1)[1] > 0
+            if self.tool is not None:
+                hit |= sim.closest_points(self.tool, ob, 0.0, max_pts=1)[1] > 0
         return hit
 
-    def toc_search(self, sim, rng, goals, n_start, attempts, max_iterations):
-        """Search, place and check; sets `goals_reached` and `unresolved` (envs still colliding after the last round) and returns
+    def toc_search(self, sim, rng, goals, n_start, attempts, max_iterations, right_side=True, base_yaw=0.0):
+        """Search, place and check (base poses on the person's right at yaw 0, or with `right_side=False` on the left); sets `goals_reached` and `unresolved` (envs still colliding after the last round) and returns
         base position, base orientation, start joint angles and the tool's position."""
         n, R = sim.n, self.R
         base0 = np.array([-0.85, -0.4, 0]) + np.array(R['toc_base_pos_offset'])
@@ -171,7 +175,7 @@ class TocPlacement:
         todo = np.ones(n, dtype=bool)
         for _ in range(max_iterations):                                          # env.py:282
             bp, bq, bj, num, _man = position_robot_toc(sim, rng, self.robot, self.arm_links, self.ee_link, self.kin, np.array(R['arm']) + 1,
-                                                       R['ee'] + 1, self.arm_lower, self.arm_upper, base0, goals, right_side=True, base_yaw=0.0,
+                                                       R['ee'] + 1, self.arm_lower, self.arm_upper, base0, goals, right_side=right_side, base_yaw=base_yaw,
                                                        attempts=attempts, mask=todo, default_q=R['default_q'], n_start=n_start)
             base_pos[todo], base_quat[todo], q7[todo], reached[todo] = bp[todo], bq[todo], bj[todo], num[todo]
             sp = self.place_robot(sim, base_pos, base_quat, q7)
