@@ -18,6 +18,8 @@ from ..dressing_batch import L_ELBOW, L_SHOULDER, L_WRIST, RADII, TRIANGLE1, TRI
 from ..sim import BatchSim
 from .env import AssistiveEnv
 
+ARM_LINKS = (L_SHOULDER, L_ELBOW, L_WRIST)
+
 
 def dressing_batch_for(robot, controllable_person=False):
     """The batched scene of `robot`'s Dressing id: PR2 or Sawyer placed by TOC, or the wheelchair-mounted Jaco."""
@@ -41,27 +43,12 @@ class DressingEnv(AssistiveEnv):
 
     def step(self, action):                                                # dressing.py:12-77
         if self.human.controllable:               # dict in, dicts out (dressing.py:16-17,73-77)
-            a = np.concatenate([np.asarray(action['robot'], dtype=np.float64).reshape(self.n_envs, -1),
-                                np.asarray(action['human'], dtype=np.float64).reshape(self.n_envs, -1)], axis=1)
-            obs, reward, done, info = self.step_reference_api(a)
-            d = bool(np.all(done)) if self.n_envs > 1 else bool(done)
-            return obs, {'robot': reward, 'human': reward}, {'robot': done, 'human': done, '__all__': d}, {'robot': info, 'human': info}
-        a = np.asarray(action, dtype=np.float32).reshape(self.n_envs, -1)
-        obs, rew, done, info = self.id.dressing_step_host(a)
-        self.iteration += 1
-        self.total_force_on_human, self.cloth_force_sum = info[:, 0], obs[:, 23]
+            return self._coop_step(action)
+        obs, rew, done, info = self._fused_step(self.id.dressing_step_host, action)
+        self.cloth_force_sum = obs[:, 23]
         self.task_success = np.maximum(self.task_success, info[:, 2])
         self.forearm_in_sleeve, self.upperarm_in_sleeve = (info[:, 3].astype(int) & 1) > 0, (info[:, 3].astype(int) & 2) > 0
-        out = {'total_force_on_human': info[:, 0], 'task_success': info[:, 1].astype(int), 'action_robot_len': self.action_robot_len,
-               'action_human_len': self.action_human_len, 'obs_robot_len': self.obs_robot_len, 'obs_human_len': self.obs_human_len}
-        if self.n_envs == 1:
-            return obs[0], float(rew[0]), bool(done[0] > 0.5), {k_: (v[0] if isinstance(v, np.ndarray) else v) for k_, v in out.items()}
-        return obs, rew, done > 0.5, out
-
-    def step_fused(self, action):
-        """`step` of the co-optimisation env (DressingPR2Human-v1) on the fused, graph-replayed device path: takes and returns
-        exactly what `step` does.  `step` itself stays on the per-call path."""
-        return self._coop_step_fused(action)
+        return self._unwrap(obs, rew, done, self._info(info[:, 0], info[:, 1].astype(int)))
 
     # ------------------------------------------------------------------ the same step through the reference-shaped API
     def step_reference_api(self, action):
@@ -71,7 +58,7 @@ class DressingEnv(AssistiveEnv):
         self.take_step(a)
         n = self.n_envs
         x, _ = self.id.cloth_get_state()
-        limb = [p_.astype(np.float64) for p_ in self._arm_points()]
+        limb = [self._person_pose(link)[0].astype(np.float64) for link in ARM_LINKS]
         forearm, upperarm, reward_dressing = np.zeros(n, dtype=bool), np.zeros(n, dtype=bool), np.zeros(n)
         for e in range(n):
             radii = RADII['male' if self.male[e] else 'female']
@@ -91,27 +78,14 @@ class DressingEnv(AssistiveEnv):
         reward = self.config('dressing_reward_weight') * reward_dressing + self.config('action_weight') * (-np.linalg.norm(a, axis=1)) + pref
         self.task_success = np.maximum(self.task_success, reward_dressing)
         done = np.full(n, self.iteration >= 200)
-        info = {'total_force_on_human': self.total_force_on_human, 'task_success': (self.task_success >= self.config('task_success_threshold')).astype(int),
-                'action_robot_len': self.action_robot_len, 'action_human_len': self.action_human_len, 'obs_robot_len': self.obs_robot_len, 'obs_human_len': self.obs_human_len}
-        if n == 1:
-            obs = {k_: v[0] for k_, v in obs.items()} if isinstance(obs, dict) else obs[0]
-            return obs, float(reward[0]), bool(done[0]), {k_: (v[0] if isinstance(v, np.ndarray) else v) for k_, v in info.items()}
-        return obs, reward, done, info
-
-    def _arm_points(self):
-        out = []
-        for link in (L_SHOULDER, L_ELBOW, L_WRIST):
-            pm = np.atleast_2d(self.humans['male'].get_pos_orient(link)[0])
-            pf = np.atleast_2d(self.humans['female'].get_pos_orient(link)[0])
-            out.append(np.where(self.male[:, None], pm, pf))
-        return out
+        return self._unwrap(obs, reward, done, self._info(self.total_force_on_human, (self.task_success >= self.config('task_success_threshold')).astype(int)))
 
     def _get_obs(self, agent=None):                                        # dressing.py:79-106
         ep, eq = (np.atleast_2d(x) for x in self.robot.get_pos_orient(self.robot.left_end_effector))
         ep_r, eq_r = (np.atleast_2d(x) for x in self.robot.convert_to_realworld(ep, eq))
         q = np.atleast_2d(self.robot.get_joint_angles(self.robot.controllable_joint_indices))
         q = (q + np.pi) % (2 * np.pi) - np.pi
-        arm = [np.atleast_2d(self.robot.convert_to_realworld(p_)[0]) for p_ in self._arm_points()]
+        arm = [np.atleast_2d(self.robot.convert_to_realworld(self._person_pose(link)[0])[0]) for link in ARM_LINKS]
         cnt, _node, pos, force, _link = self.id.cloth_get_contacts(1024)
         f = np.linalg.norm(force * 10.0, axis=2)
         keep = (np.arange(f.shape[1])[None, :] < cnt[:, None]) & (pos[:, :, 2] < ep[:, 2:3] - 0.05) & (f < 20)
@@ -122,16 +96,9 @@ class DressingEnv(AssistiveEnv):
         if agent == 'robot' or not self.human.controllable:
             return robot_obs
         # dressing.py:96-105: the end effector, the person's joint angles (not wrapped) and the arm points in the person's base frame
-        def human_frame(pos, orient=None):
-            outs = []
-            for g in ('male', 'female'):
-                r = self.humans[g].convert_to_realworld(pos, orient if orient is not None else np.array([0, 0, 0, 1.0]))
-                outs.append([np.atleast_2d(x) for x in r])
-            return [np.where(self.male[:, None], m, f) for m, f in zip(*outs)]
-        ci = self.human.controllable_joint_indices
-        qh = np.where(self.male[:, None], np.atleast_2d(self.humans['male'].get_joint_angles(ci)), np.atleast_2d(self.humans['female'].get_joint_angles(ci)))
-        ep_h, eq_h = human_frame(ep, eq)
-        arm_h = [human_frame(p_)[0] for p_ in self._arm_points()]
+        qh = self._person_joint_angles()
+        ep_h, eq_h = self._person_frame(ep, eq)
+        arm_h = [self._person_frame(self._person_pose(link)[0])[0] for link in ARM_LINKS]
         human_obs = np.concatenate([ep_h, eq_h, qh] + arm_h + [self.cloth_force_sum[:, None], self.robot_force_on_human[:, None]], axis=1)
         if agent == 'human':
             return human_obs
@@ -141,16 +108,7 @@ class DressingEnv(AssistiveEnv):
         super().reset()
         db = self._db
         if self.id is None:
-            self.id = BatchSim(db.scene, self._cfg, self.n_envs, device=self.device, _lib=self._sim_lib)
-            sim = self.id
-            self.plane.init(db.plane, sim, self.np_random, indices=-1)
-            self.robot.init(db.robot, sim, self.np_random)
-            self.furniture.init(db.wheelchair, sim, self.np_random, indices=-1)
-            self.humans = {}
-            for g, hb in db.humans.items():
-                h = type(self.human)(self.human.controllable_joint_indices, controllable=self.human.controllable)
-                h.init(hb, sim, self.np_random, self.human.controllable_joint_indices)
-                self.humans[g] = h
+            self._attach(db, db.wheelchair, BatchSim)
         rng = np.random.default_rng(self.np_random.randint(0, 2 ** 31 - 1))
         self.agents = [self.robot]
         self.robot.motor_gains = self.human.motor_gains = 0.01             # dressing.py:117
@@ -158,21 +116,15 @@ class DressingEnv(AssistiveEnv):
         self.male = s['male'].astype(bool)
         self.human.gender = 'male' if self.male[0] else 'female'
         self.start_ee_pos = db.start_ee_pos
-        if self.human.controllable:               # both gender instances act; the switched-off one moves nothing (env.py:130)
-            for g, h in self.humans.items():
-                h.env_mask = self.male if g == 'male' else ~self.male
-                h.arm_previous_valid_pose = {True: None, False: None}
+        if self.human.controllable:               # the start pose is not clipped to the scaled limits here, unlike ScratchItch's and BedBathing's
+            self._controllable_person(s['limit_scale'])
+            for h in self.humans.values():
                 h.motor_gains, h.motor_forces = 0.01, 1.0                         # dressing.py:121; Human.motor_forces
-                h.set_limit_scale(s['limit_scale'])                               # impairment 'limits': scaled joint limits (human.py:85)
-                self.agents.append(h)
         db.start_fused(self.id, s)
         if self.human.controllable:
             db.start_coop(self.id, s)
         self.task_success = np.zeros(self.n_envs)
-        obs = self._get_obs()
-        if isinstance(obs, dict):
-            return {k_: (v[0] if self.n_envs == 1 else v) for k_, v in obs.items()}
-        return obs[0] if self.n_envs == 1 else obs
+        return self._squeeze(self._get_obs())
 
     def update_targets(self):                                              # dressing.py:200-210
         if self.human.controllable:

@@ -48,8 +48,7 @@ class DrinkingEnv(AssistiveEnv):
         super().reset()
         db = self._db
         if self.id is None:
-            self.id = BatchSim(db.scene, self._cfg, self.n_envs, device=self.device, _lib=self._sim_lib)
-            self.attach(self.id)
+            self.attach(None)
         rng = np.random.default_rng(self.np_random.randint(0, 2 ** 31 - 1))
         s = db.reset(self.id, rng, settle_steps=50, impairment='no_tremor')
         self.start_episode(s)
@@ -57,22 +56,12 @@ class DrinkingEnv(AssistiveEnv):
         return self._squeeze(self._get_obs())
 
     def attach(self, sim):
-        """the Agent objects of the scene on `sim` (any object with the BatchSim getter / setter surface)"""
-        db = self._db
-        self.id = sim
-        self.plane.init(db.plane, sim, self.np_random, indices=-1)
-        self.robot.init(db.robot, sim, self.np_random)
-        self.tool.init(db.tool, sim, self.np_random, indices=-1)
-        self.furniture.init(db.wheelchair, sim, self.np_random, indices=-1)
-        self.humans = {}
-        for g, hb in db.humans.items():
-            h = type(self.human)(self.human.controllable_joint_indices, controllable=False)
-            h.init(hb, sim, self.np_random, self.human.controllable_joint_indices)
-            self.humans[g] = h
+        """the Agent objects of the scene on `sim` (any object with the BatchSim getter / setter surface; None: a new BatchSim)"""
+        self._attach(self._db, self._db.wheelchair, BatchSim, sim)
         self.water_agents = []
-        for w in db.waters:
+        for w in self._db.waters:
             a = Agent()
-            a.init(w, sim, self.np_random, indices=-1)
+            a.init(w, self.id, self.np_random, indices=-1)
             self.water_agents.append(a)
 
     def start_episode(self, s):
@@ -88,9 +77,6 @@ class DrinkingEnv(AssistiveEnv):
         self.task_success = np.zeros(self.n_envs, dtype=int)
         self.iteration = 0
         self.update_targets()
-
-    def _squeeze(self, a):
-        return a[0] if self.n_envs == 1 else a
 
     # ------------------------------------------------------------------ step (drinking.py:10-49)
     def step(self, action):
@@ -108,39 +94,22 @@ class DrinkingEnv(AssistiveEnv):
         reward = (self.config('distance_weight') * reward_distance + self.config('action_weight') * (-np.linalg.norm(a, axis=1)) +
                   self.config('cup_tilt_weight') * reward_tilt + self.config('drinking_reward_weight') * reward_water + pref)
         done = np.full(self.n_envs, self.iteration >= 200)
-        info = {'total_force_on_human': self.total_force_on_human, 'task_success': (self.task_success >= self.total_water_count * self.config('task_success_threshold')).astype(int),
-                'action_robot_len': self.action_robot_len, 'action_human_len': self.action_human_len, 'obs_robot_len': self.obs_robot_len, 'obs_human_len': self.obs_human_len}
-        if self.n_envs == 1:
-            return obs[0], float(reward[0]), bool(done[0]), {k_: (v[0] if isinstance(v, np.ndarray) else v) for k_, v in info.items()}
-        return obs, reward, done, info
+        return self._unwrap(obs, reward, done, self._info(self.total_force_on_human, (self.task_success >= self.total_water_count * self.config('task_success_threshold')).astype(int)))
 
     def step_fused(self, action):
-        """`step` on the fused, graph-replayed device path (armed by `reset`): takes and returns exactly what `step` does, and
-        leaves `waters`, `waters_active` and `task_success` as `step` would."""
-        a = np.asarray(action, dtype=np.float32).reshape(self.n_envs, -1)
-        obs, rew, done, info = self.id.drinking_step_host(a)
-        self.iteration += 1
+        """`step` on the fused, graph-replayed device path (armed by `reset`): takes and returns exactly what `step` does (float64
+        obs and reward, unlike the other tasks' fused steps), and leaves `waters`, `waters_active` and `task_success` as `step` would."""
+        obs, rew, done, info = self._fused_step(self.id.drinking_step_host, action)
         ts, w, wa = self.id.drinking_get_state()
         bits = np.arange(N_WATER, dtype=np.uint64)
         self.waters = ((w[:, None] >> bits) & np.uint64(1)).astype(bool)
         self.waters_active = ((wa[:, None] >> bits) & np.uint64(1)).astype(bool)
         self.task_success = ts.astype(int)
         self.total_force_on_human, self.robot_force_on_human, self.cup_force_on_human = (info[:, k].astype(np.float64) for k in (0, 2, 3))
-        obs, reward, done = obs.astype(np.float64), rew.astype(np.float64), done > 0.5
-        info = {'total_force_on_human': self.total_force_on_human, 'task_success': info[:, 1].astype(int),
-                'action_robot_len': self.action_robot_len, 'action_human_len': self.action_human_len, 'obs_robot_len': self.obs_robot_len, 'obs_human_len': self.obs_human_len}
-        if self.n_envs == 1:
-            return obs[0], float(reward[0]), bool(done[0]), {k_: (v[0] if isinstance(v, np.ndarray) else v) for k_, v in info.items()}
-        return obs, reward, done, info
-
-    def _head_pose(self):
-        pm, qm = self.humans['male'].get_pos_orient(HEAD_LINK)
-        pf, qf = self.humans['female'].get_pos_orient(HEAD_LINK)
-        pm, qm, pf, qf = (np.atleast_2d(x) for x in (pm, qm, pf, qf))
-        return np.where(self.male[:, None], pm, pf), np.where(self.male[:, None], qm, qf)
+        return self._unwrap(obs.astype(np.float64), rew.astype(np.float64), done, self._info(self.total_force_on_human, info[:, 1].astype(int)))
 
     def update_targets(self):                                            # drinking.py:192-196
-        hp, hq = self._head_pose()
+        hp, hq = self._person_pose(HEAD_LINK)
         self.target_pos = hp + q_rot(hq, self.mouth_pos)
 
     def _cup_centres(self):                                              # drinking.py:24-26, 54-57
@@ -158,7 +127,7 @@ class DrinkingEnv(AssistiveEnv):
         cp_r, cq_r = (np.atleast_2d(x) for x in self.robot.convert_to_realworld(cp, cq))
         q = np.atleast_2d(self.robot.get_joint_angles(self.robot.controllable_joint_indices))
         q = (q + np.pi) % (2 * np.pi) - np.pi
-        hp, hq = self._head_pose()
+        hp, hq = self._person_pose(HEAD_LINK)
         hp_r, hq_r = (np.atleast_2d(x) for x in self.robot.convert_to_realworld(hp, hq))
         tg_r = np.atleast_2d(self.robot.convert_to_realworld(self.target_pos)[0])
         self.robot_force_on_human, self.cup_force_on_human = self.get_total_force()

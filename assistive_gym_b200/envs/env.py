@@ -208,10 +208,92 @@ class AssistiveEnv(gym.Env):
     def update_targets(self):
         pass
 
-    def _coop_step_fused(self, action):
+    # ---- what every task env shares around its own observation and reward code
+    def _attach(self, batch, furniture, sim_type, sim=None):
+        """The Agent objects of `batch`'s scene on `sim` (any object with the BatchSim getter / setter surface; by default a new
+        `sim_type` of the scene): the plane, the robot, the tool when the scene has one, `furniture` and both genders' `Human`.
+        `sim_type` is the `BatchSim` of the task's module, looked up when the env is reset, so that a test can put the CPU oracle
+        in its place."""
+        self.id = sim if sim is not None else sim_type(batch.scene, self._cfg, self.n_envs, device=self.device, _lib=self._sim_lib)
+        self.plane.init(batch.plane, self.id, self.np_random, indices=-1)
+        self.robot.init(batch.robot, self.id, self.np_random)
+        if batch.tool is not None:
+            self.tool.init(batch.tool, self.id, self.np_random, indices=-1)
+        self.furniture.init(furniture, self.id, self.np_random, indices=-1)
+        self.humans = {}
+        for g, hb in batch.humans.items():
+            h = type(self.human)(self.human.controllable_joint_indices, controllable=self.human.controllable)
+            h.init(hb, self.id, self.np_random, self.human.controllable_joint_indices)
+            self.humans[g] = h
+
+    def _controllable_person(self, limit_scale):
+        """Both gender instances of the person act; the switched-off one moves nothing (env.py:130).  `limit_scale`: the per-env
+        joint-limit scale of impairment 'limits' (human.py:85)."""
+        for g, h in self.humans.items():
+            h.env_mask = self.male if g == 'male' else ~self.male
+            h.arm_previous_valid_pose = {True: None, False: None}
+            h.set_limit_scale(limit_scale)
+            self.agents.append(h)
+
+    def _person_pose(self, link):
+        """world position [n, 3] and orientation [n, 4] of `link` of each env's person (the gender instance `self.male` selects)"""
+        pm, qm = (np.atleast_2d(x) for x in self.humans['male'].get_pos_orient(link))
+        pf, qf = (np.atleast_2d(x) for x in self.humans['female'].get_pos_orient(link))
+        return np.where(self.male[:, None], pm, pf), np.where(self.male[:, None], qm, qf)
+
+    def _person_frame(self, pos, orient=None):
+        """[pos, orient] in each env's person's base frame"""
+        outs = []
+        for g in ('male', 'female'):
+            r = self.humans[g].convert_to_realworld(pos, orient if orient is not None else np.array([0, 0, 0, 1.0]))
+            outs.append([np.atleast_2d(x) for x in r])
+        return [np.where(self.male[:, None], m, f) for m, f in zip(*outs)]
+
+    def _person_joint_angles(self):
+        """the controllable joint angles of each env's person, [n, k]"""
+        ci = self.human.controllable_joint_indices
+        return np.where(self.male[:, None], np.atleast_2d(self.humans['male'].get_joint_angles(ci)), np.atleast_2d(self.humans['female'].get_joint_angles(ci)))
+
+    def _info(self, total_force_on_human, task_success):
+        return {'total_force_on_human': total_force_on_human, 'task_success': task_success, 'action_robot_len': self.action_robot_len,
+                'action_human_len': self.action_human_len, 'obs_robot_len': self.obs_robot_len, 'obs_human_len': self.obs_human_len}
+
+    def _squeeze(self, a):
+        """env 0's value (of every entry of a dict) when n_envs == 1"""
+        if isinstance(a, dict):
+            return {k: self._squeeze(v) for k, v in a.items()}
+        return a[0] if self.n_envs == 1 else a
+
+    def _unwrap(self, obs, reward, done, info):
+        """`step`'s return with n_envs == 1: env 0's observation, a float reward, a bool done and env 0's info values"""
+        if self.n_envs > 1:
+            return obs, reward, done, info
+        return self._squeeze(obs), float(reward[0]), bool(done[0]), {k: (v[0] if isinstance(v, np.ndarray) else v) for k, v in info.items()}
+
+    def _by_agent(self, obs, reward, done, info):
+        """the co-optimisation `step`'s return: the step's reward, done and info for both agents, and '__all__'"""
+        d = bool(np.all(done)) if self.n_envs > 1 else bool(done)
+        return obs, {'robot': reward, 'human': reward}, {'robot': done, 'human': done, '__all__': d}, {'robot': info, 'human': info}
+
+    def _coop_step(self, action):
+        """`step` with a controllable person, on the per-call path: {'robot': a, 'human': a_h} through `step_reference_api`"""
+        n = self.n_envs
+        a = np.concatenate([np.asarray(action['robot'], dtype=np.float64).reshape(n, -1), np.asarray(action['human'], dtype=np.float64).reshape(n, -1)], axis=1)
+        return self._by_agent(*self.step_reference_api(a))
+
+    def _fused_step(self, step_host, action):
+        """One single-agent step on the fused device path (`step_host`, e.g. `self.id.feeding_step_host`): obs [n, obs_robot_len]
+        float32, reward [n] float32, done [n] bool and the raw info [n, 4] (force on the person, task success, two task columns)."""
+        obs, rew, done, info = step_host(np.asarray(action, dtype=np.float32).reshape(self.n_envs, -1))
+        self.iteration += 1
+        self.total_force_on_human = info[:, 0]
+        return obs, rew, done > 0.5, info
+
+    def step_fused(self, action):
         """The co-optimisation step (dict action in, dict observations / rewards / dones / infos out, as `step` returns them with a
         controllable person) on the fused device path: robot and person act, the person's limits and the realistic-arm-limit
-        classifier run on the device after every substep (ag_coop_step_host).  Armed by `reset` (`start_coop`)."""
+        classifier run on the device after every substep (ag_coop_step_host).  Armed by `reset` (`start_coop`).  `step` itself
+        stays on the per-call path."""
         if not (self.human is not None and self.human.controllable):
             raise RuntimeError('step_fused is the co-optimisation step: this env has no controllable person')
         n = self.n_envs
@@ -219,13 +301,8 @@ class AssistiveEnv(gym.Env):
         obs_r, obs_h, rew, done, info = self.id.coop_step_host(a)
         self.iteration += 1
         self.total_force_on_human = info[:, 0].astype(np.float64)
-        sq = (lambda v: v[0] if n == 1 else v)
-        obs = {'robot': sq(obs_r.astype(np.float64)), 'human': sq(obs_h.astype(np.float64))}
-        reward, done = sq(rew.astype(np.float64)), sq(done > 0.5)
-        inf = {'total_force_on_human': self.total_force_on_human, 'task_success': info[:, 1].astype(int),
-               'action_robot_len': self.action_robot_len, 'action_human_len': self.action_human_len, 'obs_robot_len': self.obs_robot_len, 'obs_human_len': self.obs_human_len}
-        d = bool(np.all(done)) if n > 1 else bool(done)
-        return obs, {'robot': reward, 'human': reward}, {'robot': done, 'human': done, '__all__': d}, {'robot': inf, 'human': inf}
+        obs = self._squeeze({'robot': obs_r.astype(np.float64), 'human': obs_h.astype(np.float64)})
+        return self._by_agent(obs, self._squeeze(rew.astype(np.float64)), self._squeeze(done > 0.5), self._info(self.total_force_on_human, info[:, 1].astype(int)))
 
     # ---- env.py:237-274
     def human_preferences(self, end_effector_velocity=0, total_force_on_human=0, tool_force_at_target=0, food_hit_human_reward=0,

@@ -42,26 +42,15 @@ class FeedingEnv(AssistiveEnv):
         super().reset()
         fb = self._fb
         if self.id is None:
-            self.id = BatchSim(fb.scene, self._cfg, self.n_envs, device=self.device, _lib=self._sim_lib)
-            sim = self.id
-            self.plane.init(fb.plane, sim, self.np_random, indices=-1)
-            self.robot.init(fb.robot, sim, self.np_random)
-            self.tool.init(fb.tool, sim, self.np_random, indices=-1)
-            self.furniture.init(fb.wheelchair, sim, self.np_random, indices=-1)
+            self._attach(fb, fb.wheelchair, BatchSim)
             self.table, self.bowl = Furniture(), Furniture()
-            self.table.init(fb.table, sim, self.np_random, indices=-1)
-            self.bowl.init(fb.bowl, sim, self.np_random, indices=-1)
-            self.humans = {}
-            for g, hb in fb.humans.items():
-                h = type(self.human)(self.human.controllable_joint_indices, controllable=self.human.controllable)
-                h.init(hb, sim, self.np_random, self.human.controllable_joint_indices)
-                self.humans[g] = h
+            self.table.init(fb.table, self.id, self.np_random, indices=-1)
+            self.bowl.init(fb.bowl, self.id, self.np_random, indices=-1)
             self.foods_agents = []
             for f in fb.foods:
                 a = Agent()
-                a.init(f, sim, self.np_random, indices=-1)
+                a.init(f, self.id, self.np_random, indices=-1)
                 self.foods_agents.append(a)
-            self._feeding_ready = False
         rng = np.random.default_rng(self.np_random.randint(0, 2 ** 31 - 1))
         self.robot.motor_gains = self.human.motor_gains = 0.025          # feeding.py:122
         self.agents = [self.robot]
@@ -90,11 +79,7 @@ class FeedingEnv(AssistiveEnv):
                 h.motor_gains, h.motor_forces = self.human.motor_gains, self.human.motor_forces
                 self.agents.append(h)
         self.mouth_pos = np.where(self.male[:, None], fb.mouth['male'], fb.mouth['female'])
-        if not self._feeding_ready:
-            fb.start_fused(self.id, s, seed=self._seed)
-            self._feeding_ready = True
-        else:
-            fb.start_fused(self.id, s, seed=self._seed)
+        fb.start_fused(self.id, s, seed=self._seed)
         if coop:
             fb.start_coop(self.id, s)
         self.foods = np.ones((self.n_envs, 8), dtype=bool)
@@ -103,43 +88,18 @@ class FeedingEnv(AssistiveEnv):
         self.update_targets()
         return self._squeeze(self._get_obs())
 
-    def _squeeze(self, a):
-        if isinstance(a, dict):
-            return {k: self._squeeze(v) for k, v in a.items()}
-        return a[0] if self.n_envs == 1 else a
-
     # ------------------------------------------------------------------ fused step (feeding.py:12-43)
     def step(self, action):
         if self.human.controllable:               # feeding.py:13-14,40-43: dict in, dicts out (per-call API path)
-            a = np.concatenate([np.asarray(action['robot'], dtype=np.float64).reshape(self.n_envs, -1), np.asarray(action['human'], dtype=np.float64).reshape(self.n_envs, -1)], axis=1)
-            obs, reward, done, info = self.step_reference_api(a)
-            d = bool(np.all(done)) if self.n_envs > 1 else bool(done)
-            return obs, {'robot': reward, 'human': reward}, {'robot': done, 'human': done, '__all__': d}, {'robot': info, 'human': info}
-        a = np.asarray(action, dtype=np.float32).reshape(self.n_envs, -1)
-        obs, rew, done, info = self.id.feeding_step_host(a)
-        self.iteration += 1
-        self.total_force_on_human = info[:, 0]
-        infos = [{'total_force_on_human': float(info[e, 0]), 'task_success': int(info[e, 1]), 'action_robot_len': self.action_robot_len,
-                  'action_human_len': self.action_human_len, 'obs_robot_len': self.obs_robot_len, 'obs_human_len': self.obs_human_len}
-                 for e in range(self.n_envs)]
-        if self.n_envs == 1:
-            return obs[0], float(rew[0]), bool(done[0] > 0.5), infos[0]
-        return obs, rew, done > 0.5, infos
-
-    def step_fused(self, action):
-        """`step` of the co-optimisation env (FeedingJacoHuman-v1) on the fused, graph-replayed device path: takes and returns
-        exactly what `step` does.  `step` itself stays on the per-call path."""
-        return self._coop_step_fused(action)
+            return self._coop_step(action)
+        obs, rew, done, info = self._fused_step(self.id.feeding_step_host, action)
+        # unlike the other tasks' steps, a list of per-env info dicts of Python scalars
+        infos = [self._info(float(info[e, 0]), int(info[e, 1])) for e in range(self.n_envs)]
+        return self._unwrap(obs, rew, done, infos if self.n_envs > 1 else infos[0])
 
     # ------------------------------------------------------------------ the same step through the reference-shaped API
-    def _head_pose(self):
-        pm, qm = self.humans['male'].get_pos_orient(HEAD_LINK)
-        pf, qf = self.humans['female'].get_pos_orient(HEAD_LINK)
-        pm, qm, pf, qf = (np.atleast_2d(x) for x in (pm, qm, pf, qf))
-        return np.where(self.male[:, None], pm, pf), np.where(self.male[:, None], qm, qf)
-
     def update_targets(self):                                            # feeding.py:192-196
-        hp, hq = self._head_pose()
+        hp, hq = self._person_pose(HEAD_LINK)
         self.target_pos = hp + q_rot(hq, self.mouth_pos)
 
     def get_total_force(self):                                           # feeding.py:45-48
@@ -152,7 +112,7 @@ class FeedingEnv(AssistiveEnv):
         sp_r, sq_r = (np.atleast_2d(x) for x in self.robot.convert_to_realworld(sp, sq))
         q = np.atleast_2d(self.robot.get_joint_angles(self.robot.controllable_joint_indices))
         q = (q + np.pi) % (2 * np.pi) - np.pi
-        hp, hq = self._head_pose()
+        hp, hq = self._person_pose(HEAD_LINK)
         hp_r, hq_r = (np.atleast_2d(x) for x in self.robot.convert_to_realworld(hp, hq))
         tg_r = np.atleast_2d(self.robot.convert_to_realworld(self.target_pos)[0])
         self.robot_force_on_human, self.spoon_force_on_human = self.get_total_force()
@@ -161,17 +121,10 @@ class FeedingEnv(AssistiveEnv):
         if agent == 'robot' or not self.human.controllable:
             return robot_obs
         # feeding.py:101-111: the same quantities in the person's base frame + the person's joint angles
-        def human_frame(pos, orient=None):
-            outs = []
-            for g in ('male', 'female'):
-                r = self.humans[g].convert_to_realworld(pos, orient if orient is not None else np.array([0, 0, 0, 1.0]))
-                outs.append([np.atleast_2d(x) for x in r])
-            return [np.where(self.male[:, None], m, f) for m, f in zip(*outs)]
-        qh = np.where(self.male[:, None], np.atleast_2d(self.humans['male'].get_joint_angles(self.human.controllable_joint_indices)),
-                      np.atleast_2d(self.humans['female'].get_joint_angles(self.human.controllable_joint_indices)))
-        sp_h, sq_h = human_frame(sp, sq)
-        hp_h, hq_h = human_frame(hp, hq)
-        tg_h = human_frame(self.target_pos)[0]
+        qh = self._person_joint_angles()
+        sp_h, sq_h = self._person_frame(sp, sq)
+        hp_h, hq_h = self._person_frame(hp, hq)
+        tg_h = self._person_frame(self.target_pos)[0]
         human_obs = np.concatenate([sp_h, sq_h, sp_h - tg_h, qh, hp_h, hq_h, self.robot_force_on_human[:, None], self.spoon_force_on_human[:, None]], axis=1)
         if agent == 'human':
             return human_obs
@@ -214,6 +167,6 @@ class FeedingEnv(AssistiveEnv):
         reward = (self.config('distance_weight') * (-np.linalg.norm(self.target_pos - spoon_pos, axis=1)) +
                   self.config('action_weight') * (-np.linalg.norm(a, axis=1)) + self.config('food_reward_weight') * reward_food + pref)
         done = np.full(self.n_envs, self.iteration >= 200)
-        info = {'total_force_on_human': self.total_force_on_human, 'task_success': (self.task_success >= self.total_food_count * self.config('task_success_threshold')).astype(int),
-                'action_robot_len': self.action_robot_len, 'action_human_len': self.action_human_len, 'obs_robot_len': self.obs_robot_len, 'obs_human_len': self.obs_human_len}
+        info = self._info(self.total_force_on_human, (self.task_success >= self.total_food_count * self.config('task_success_threshold')).astype(int))
+        # as ScratchItch's, unlike Dressing's, BedBathing's and Drinking's: with n_envs == 1 the reward stays a NumPy value and info is not unwrapped
         return self._squeeze(obs), self._squeeze(reward), self._squeeze(done), info
