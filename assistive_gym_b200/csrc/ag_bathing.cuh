@@ -43,9 +43,9 @@ AG_HDN inline void bathing_dist_body(int tid, const SimDev& S, const KP& p) {
     for (int l = lt; l < lt + nlt; l++) {
       int t0 = AG_LDG(S.link_col0 + l), tn = AG_LDG(S.link_ncol + l);
       for (int ct = t0; ct < t0 + tn; ct++) {
-        NpOut out[4];
+        NpOut c;
         int ca = ct < ch ? ct : ch, cb = ct < ch ? ch : ct;
-        if (narrow_pair(S, e, ca, cb, 5.0f, false, out)) best = fminf(best, out[0].d);
+        if (narrow_closest(S, e, ca, cb, 5.0f, c)) best = fminf(best, c.d);
       }
     }
   }

@@ -108,6 +108,12 @@ AG_HDN inline void linkaabb_body(int tid, const SimDev& S, const KP& p) {
 }
 
 // ------------------------------------------------------------------ K3: narrowphase
+// AG_NARROW_STAT(event, value): a no-op, unless tools/narrow_work.py defines it on a host build to count where k_narrow's
+// work goes: each candidate pair is bracketed by `cand` (its tid) and `done` (its contacts), with GJK iterations, face-axis
+// fallbacks and the manifold pool's fill in between.
+#ifndef AG_NARROW_STAT
+#define AG_NARROW_STAT(event, value) ((void)0)
+#endif
 AG_HD bool aabb_ov(f3 amin, f3 amax, f3 bmin, f3 bmax, float m) {
   return !(amin.x > bmax.x + m || bmin.x > amax.x + m || amin.y > bmax.y + m || bmin.y > amax.y + m ||
            amin.z > bmax.z + m || bmin.z > amax.z + m);
@@ -174,18 +180,53 @@ AG_HD int support4(const float* vq, int g0, int n, f3 d) {
   return bi < n ? bi : 0;      // a pad entry can only tie with vertex 0, never beat it; guard anyway
 }
 
+// The GJK simplex: up to 4 points (support points PA / PB and their vertex indices) and their barycentric weights.  A point of
+// the Minkowski difference, w(i), is recomputed from PA / PB with the expression it was made with.  Every index into these
+// arrays is a compile-time constant once the callers' loops are unrolled: a slot known only at run time is matched against
+// each constant slot, so the simplex stays in registers.
+struct Simplex {
+  f3 PA[4], PB[4];
+  int IA[4], IB[4];
+  double lam[4];
+  AG_HD d3 w(int i) const { return to_d3(PA[i]) - to_d3(PB[i]); }
+  // w(i) for an i known only at run time
+  AG_HD d3 w_at(int i) const {
+    f3 a = PA[0], b = PB[0];
+#pragma unroll
+    for (int j = 1; j < 4; j++) if (j == i) { a = PA[j]; b = PB[j]; }
+    return to_d3(a) - to_d3(b);
+  }
+  // slot m <- the point (a, b, ia, ib)
+  AG_HD void put(int m, f3 a, f3 b, int ia, int ib) {
+#pragma unroll
+    for (int j = 0; j < 4; j++) if (j == m) { PA[j] = a; PB[j] = b; IA[j] = ia; IB[j] = ib; }
+  }
+  // slot m <- point i of `s`, with weight l
+  AG_HD void take(int m, const Simplex& s, int i, double l) {
+#pragma unroll
+    for (int j = 0; j < 4; j++) if (j == m) { PA[j] = s.PA[i]; PB[j] = s.PB[i]; IA[j] = s.IA[i]; IB[j] = s.IB[i]; lam[j] = l; }
+  }
+};
+// slot k (0..2; 3 = the opposite vertex) of face f of the tetrahedron
+AG_HD int tet_face(int f, int k) {
+  if (k == 0) return (f == 3) ? 1 : 0;
+  if (k == 1) return (f == 0) ? 1 : ((f == 1) ? 2 : 3);
+  if (k == 2) return (f == 0) ? 2 : ((f == 1) ? 3 : ((f == 2) ? 1 : 2));
+  return (f == 0) ? 3 : ((f == 1) ? 1 : ((f == 2) ? 2 : 0));
+}
+
 // `vq` / ga0, gb0: the packed copies of the two cores (group offsets); verts / va0, vb0: the plain copies
 AG_HDN inline bool gjk_cores(const float* verts, const float* vq, int va0, int ga0, int nA, int vb0, int gb0, int nB, const m3& R, f3 t,
                              f3& pa, f3& pb, f3& nrm, float& dist) {
-  d3 W[4]; f3 PA[4], PB[4];
-  int IA[4], IB[4];
-  double lam[4] = {1.0, 0.0, 0.0, 0.0};
+  Simplex sx;
+  sx.lam[0] = 1.0; sx.lam[1] = 0.0; sx.lam[2] = 0.0; sx.lam[3] = 0.0;
   int n = 0;
   d3 v = to_d3(mul(R, tv3(verts, va0)) + t) - to_d3(tv3(verts, vb0));
   if (dot(v, v) < 1e-20) v = d3(1.0, 0.0, 0.0);
   bool overlap = false;
   double lower_bound = 0.0;
   for (int it = 0; it < 32; it++) {
+    AG_NARROW_STAT(gjk_iter, it);
     // support of A in direction -v (A-local: R^T(-v)), support of B in +v
     f3 vf = to_f3(v);
     f3 da = mulT(R, -vf);
@@ -198,27 +239,28 @@ AG_HDN inline bool gjk_cores(const float* verts, const float* vq, int va0, int g
     if (n > 0 && vw > 0.0) lower_bound = fmax(lower_bound, vw / sqrt(vv));
     if (n > 0 && vv - vw <= 1e-10 * vv) break;
     bool dup = false;
-    for (int i = 0; i < n; i++) if (IA[i] == ia && IB[i] == ib) dup = true;
+#pragma unroll
+    for (int i = 0; i < 4; i++) if (i < n && sx.IA[i] == ia && sx.IB[i] == ib) dup = true;
     if (dup) break;
-    W[n] = w; PA[n] = sa; PB[n] = sb; IA[n] = ia; IB[n] = ib; n++;
-    if (n == 1) { lam[0] = 1.0; }
+    sx.put(n, sa, sb, ia, ib); n++;
+    if (n == 1) { sx.lam[0] = 1.0; }
     else if (n == 2) {
-      double u, s; seg_origin(W[0], W[1], u, s);
-      if (s <= 0.0) { n = 1; lam[0] = 1.0; }
-      else if (u <= 0.0) { W[0] = W[1]; PA[0] = PA[1]; PB[0] = PB[1]; IA[0] = IA[1]; IB[0] = IB[1]; n = 1; lam[0] = 1.0; }
-      else { lam[0] = u; lam[1] = s; }
+      double u, s; seg_origin(sx.w(0), sx.w(1), u, s);
+      if (s <= 0.0) { n = 1; sx.lam[0] = 1.0; }
+      else if (u <= 0.0) { sx.take(0, sx, 1, 1.0); n = 1; }
+      else { sx.lam[0] = u; sx.lam[1] = s; }
     } else if (n == 3) {
-      double l3[3]; tri_origin(W[0], W[1], W[2], l3[0], l3[1], l3[2]);
+      double l3[3]; tri_origin(sx.w(0), sx.w(1), sx.w(2), l3[0], l3[1], l3[2]);
       int m = 0;
-      for (int i = 0; i < 3; i++) if (l3[i] > 0.0) { W[m] = W[i]; PA[m] = PA[i]; PB[m] = PB[i]; IA[m] = IA[i]; IB[m] = IB[i]; lam[m] = l3[i]; m++; }
+#pragma unroll
+      for (int i = 0; i < 3; i++) if (l3[i] > 0.0) { sx.take(m, sx, i, l3[i]); m++; }     // m <= i: slot i is read before it is written
       n = m;
     } else {
       double bestd = 1e300; int bf = -1; double bl[3] = {0.0, 0.0, 0.0};
-      double bestd_all = 1e300; int bf_all = 0; double bla[3] = {1.0, 0.0, 0.0};
+      double bestd_all = 1e300; int bf_all = -1;
       bool any_out = false;
       for (int f = 0; f < 4; f++) {
-        int i0 = (f == 3) ? 1 : 0, i1 = (f == 0) ? 1 : ((f == 1) ? 2 : 3), i2 = (f == 0) ? 2 : ((f == 1) ? 3 : ((f == 2) ? 1 : 2)), i3 = (f == 0) ? 3 : ((f == 1) ? 1 : ((f == 2) ? 2 : 0));
-        d3 a = W[i0], b = W[i1], c = W[i2], d = W[i3];
+        d3 a = sx.w_at(tet_face(f, 0)), b = sx.w_at(tet_face(f, 1)), c = sx.w_at(tet_face(f, 2)), d = sx.w_at(tet_face(f, 3));
         d3 nn = cross(b - a, c - a);
         double sp = -dot(a, nn), sd = dot(d - a, nn);
         // inside only if CLEARLY on the opposite vertex's side; flat tetrahedra count as outside
@@ -228,7 +270,7 @@ AG_HDN inline bool gjk_cores(const float* verts, const float* vq, int va0, int g
         double u, s, r; tri_origin(a, b, c, u, s, r);
         d3 pt = a * u + b * s + c * r;
         double dd = dot(pt, pt);
-        if (dd < bestd_all) { bestd_all = dd; bf_all = f; bla[0] = u; bla[1] = s; bla[2] = r; }
+        if (dd < bestd_all) { bestd_all = dd; bf_all = f; }
         if (inside) continue;
         any_out = true;
         if (dd < bestd) { bestd = dd; bf = f; bl[0] = u; bl[1] = s; bl[2] = r; }
@@ -236,25 +278,33 @@ AG_HDN inline bool gjk_cores(const float* verts, const float* vq, int va0, int g
       if (!any_out) {
         // a positive lower bound on the distance (v.w/|v| of an earlier iteration) proves separation
         if (lower_bound <= 1e-7) { overlap = true; break; }
-        bf = bf_all; bl[0] = bla[0]; bl[1] = bla[1]; bl[2] = bla[2];
+        // the face nearest the origin, its weights recomputed as in the loop (not carried through it: register pressure)
+        bf = bf_all < 0 ? 0 : bf_all; bl[0] = 1.0; bl[1] = 0.0; bl[2] = 0.0;
+        if (bf_all >= 0) tri_origin(sx.w_at(tet_face(bf, 0)), sx.w_at(tet_face(bf, 1)), sx.w_at(tet_face(bf, 2)), bl[0], bl[1], bl[2]);
       }
-      int f = bf;
-      int id[3];
-      id[0] = (f == 3) ? 1 : 0; id[1] = (f == 0) ? 1 : ((f == 1) ? 2 : 3); id[2] = (f == 0) ? 2 : ((f == 1) ? 3 : ((f == 2) ? 1 : 2));
-      d3 tw[3]; f3 ta[3], tb[3]; int tia[3], tib[3];
-      for (int i = 0; i < 3; i++) { tw[i] = W[id[i]]; ta[i] = PA[id[i]]; tb[i] = PB[id[i]]; tia[i] = IA[id[i]]; tib[i] = IB[id[i]]; }
+      // the chosen face's points, copied out first (a face's slots are not in ascending order), then kept where bl > 0
+      Simplex fc;
+#pragma unroll
+      for (int k = 0; k < 3; k++) {
+        const int src = tet_face(bf, k);
+#pragma unroll
+        for (int j = 0; j < 4; j++) if (j == src) fc.take(k, sx, j, 0.0);
+      }
       int m = 0;
-      for (int i = 0; i < 3; i++) if (bl[i] > 0.0) { W[m] = tw[i]; PA[m] = ta[i]; PB[m] = tb[i]; IA[m] = tia[i]; IB[m] = tib[i]; lam[m] = bl[i]; m++; }
+#pragma unroll
+      for (int i = 0; i < 3; i++) if (bl[i] > 0.0) { sx.take(m, fc, i, bl[i]); m++; }
       n = m;
     }
     d3 nv(0.0, 0.0, 0.0);
-    for (int i = 0; i < n; i++) nv = nv + W[i] * lam[i];
+#pragma unroll
+    for (int i = 0; i < 4; i++) if (i < n) nv = nv + sx.w(i) * sx.lam[i];
     v = nv;
     if (dot(v, v) <= 1e-16) { overlap = true; break; }
   }
   if (overlap) return true;
   d3 qa(0.0, 0.0, 0.0), qb(0.0, 0.0, 0.0);
-  for (int i = 0; i < n; i++) { qa = qa + to_d3(PA[i]) * lam[i]; qb = qb + to_d3(PB[i]) * lam[i]; }
+#pragma unroll
+  for (int i = 0; i < 4; i++) if (i < n) { qa = qa + to_d3(sx.PA[i]) * sx.lam[i]; qb = qb + to_d3(sx.PB[i]) * sx.lam[i]; }
   d3 d = qa - qb;
   double dn = sqrt(dot(d, d));
   pa = to_f3(qa); pb = to_f3(qb);
@@ -287,28 +337,42 @@ AG_HDN inline void pen_faces(const SimDev& S, int va0, int nA, int pa0, int npA,
   dist = fminf(best, 0.f);
 }
 
-struct CandSet { NpOut c[4]; int n; };
-// keep the primary + up to 3 more, greedily the farthest from the chosen set
-struct CandSel {
-  NpOut prim; NpOut pool[12]; int np;
-};
+// Manifold candidates.  face_cands finds the supporting face of the plane owner and appends the vertices of the other core
+// that lie over it to a per-thread pool of NARROW_POOL entries: (vertex index, call) in one word, the depth, and the contact
+// points on both surfaces as computed at the test.  The normal is not stored: it is the face normal of the call that found the
+// entry (FaceRef), negated for call 1.  The points are stored rather than recomputed when read because a recomputation,
+// compiled in another context, need not contract its multiply-adds the same way, and the device's contacts would change bits.
+#define NARROW_POOL 12
+// pool words: keys [0, 12), depths [12, 24), squared distance to the chosen set [24, 36), pa [36, 72), pb [72, 108);
+// one word more so that the stride between threads is odd and a warp's accesses to the same word hit 32 distinct banks
+#define NARROW_POOL_WORDS (9 * NARROW_POOL + 1)
+// one face_cands call: the tested vertices (core V from v0, mapped by R,t into B-local coordinates when V is A), the radii of V
+// and of the plane owner, and the supporting face's plane (nf, df) in B-local coordinates
+struct FaceRef { f3 nf; float df, rV, rP; int v0; bool v_is_a; };
+AG_HD FaceRef face_ref(int v0, bool v_is_a, float rV, float rP) {
+  FaceRef F; F.nf = f3(0.f, 0.f, 0.f); F.df = 0.f; F.rV = rV; F.rP = rP; F.v0 = v0; F.v_is_a = v_is_a; return F;
+}
 
 // vertices of core V that lie over the supporting face of the plane owner (see oracle for the rule).
-// Everything in B-local coordinates; `planes are given by (p0, np, xf)` where xf says whether plane
-// normals need mapping by R,t (owner is A) or not (owner is B).
-AG_HDN inline void face_cands(const SimDev& S, int vv0, int nV, float rV, bool v_is_a, int p0, int np, float rP,
-                              const m3& R, f3 t, f3 n_to_v, float d_primary, float tol, float max_dist, CandSel& cs) {
+// Everything in B-local coordinates; the planes (p0, np) are mapped by R,t when their owner is A (F.v_is_a false).
+// `call` (0 or 1) is stored with each entry put into `pool` (np_pool entries so far).
+AG_HDN inline void face_cands(const SimDev& S, int call, FaceRef& F, int nV, int p0, int np, const m3& R, f3 t, f3 n_to_v,
+                              float d_primary, float tol, float max_dist, float* pool, int& np_pool) {
+  int* pkey = (int*)pool;
+  float* pd = pool + NARROW_POOL;
+  const bool v_is_a = F.v_is_a;
   // supporting face
-  int kf = -1; float best = 0.98f; f3 nf; float df = 0.f;
+  int kf = -1; float best = 0.98f;
   for (int k = 0; k < np; k++) {
     f3 n; float d; ld_plane(S.planes, p0 + k, n, d);
     if (!v_is_a) { f3 nw = mul(R, n); d = d + dot(nw, t); n = nw; }   // plane owner is A: map to B-local
     float al = dot(n, n_to_v);
-    if (al > best) { best = al; kf = k; nf = n; df = d; }
+    if (al > best) { best = al; kf = k; F.nf = n; F.df = d; }
   }
   if (kf < 0) return;
+  const f3 nf = F.nf; const float df = F.df, rV = F.rV, rP = F.rP;
   for (int i = 0; i < nV; i++) {
-    f3 v = tv3(S.verts, vv0 + i);
+    f3 v = tv3(S.verts, F.v0 + i);
     if (v_is_a) v = mul(R, v) + t;
     float h = dot(nf, v) - df;
     float d = h - rV - rP;
@@ -322,50 +386,54 @@ AG_HDN inline void face_cands(const SimDev& S, int vv0, int nV, float rV, bool v
       if (dot(n, proj) - dd > 1e-6f) { inside = false; break; }
     }
     if (!inside) continue;
-    if (cs.np >= 12) {
+    int q = np_pool;
+    if (np_pool >= NARROW_POOL) {
       // pool full: replace the shallowest entry if this one is deeper
-      int wi = 0; for (int q = 1; q < 12; q++) if (cs.pool[q].d > cs.pool[wi].d) wi = q;
-      if (d >= cs.pool[wi].d) continue;
-      cs.np = 12;
-      NpOut& o = cs.pool[wi];
-      f3 on_v = v - nf * rV, on_f = proj + nf * rP;
-      if (v_is_a) { o.pa = on_v; o.pb = on_f; o.n = nf; } else { o.pa = on_f; o.pb = on_v; o.n = -nf; }
-      o.d = d;
-      continue;
+      q = 0; for (int r = 1; r < NARROW_POOL; r++) if (pd[r] > pd[q]) q = r;
+      if (d >= pd[q]) continue;
+    } else {
+      np_pool++;
     }
-    NpOut& o = cs.pool[cs.np++];
     f3 on_v = v - nf * rV, on_f = proj + nf * rP;
-    if (v_is_a) { o.pa = on_v; o.pb = on_f; o.n = nf; } else { o.pa = on_f; o.pb = on_v; o.n = -nf; }
-    o.d = d;
+    f3 pa = v_is_a ? on_v : on_f, pb = v_is_a ? on_f : on_v;
+    pkey[q] = (i << 1) | call;
+    pd[q] = d;
+    float* ppa = pool + 3 * NARROW_POOL + 3 * q;
+    float* ppb = pool + 6 * NARROW_POOL + 3 * q;
+    ppa[0] = pa.x; ppa[1] = pa.y; ppa[2] = pa.z;
+    ppb[0] = pb.x; ppb[1] = pb.y; ppb[2] = pb.z;
   }
 }
 
-// Manifold selection.  The GJK primary point is arbitrary within a flat contact patch (any point of
-// two parallel faces is "closest"), so whenever feature candidates exist the manifold is built from
-// them only: deepest candidate first, then greedily the candidate farthest from the chosen set.
-AG_HDN inline int select_cands(const CandSel& cs, NpOut* out) {
-  if (cs.np == 0) { out[0] = cs.prim; return 1; }
-  bool used[12];
-  int first = 0;
-  for (int i = 0; i < 12; i++) used[i] = i >= cs.np;
-  for (int i = 1; i < cs.np; i++) if (cs.pool[i].d < cs.pool[first].d) first = i;
-  int nc = 0; out[nc++] = cs.pool[first]; used[first] = true;
-  while (nc < 4) {
-    int bi = -1; float bd = 1e-8f;
-    for (int i = 0; i < cs.np; i++) {
-      if (used[i]) continue;
-      float md = 1e30f;
-      for (int k = 0; k < nc; k++) { f3 d = cs.pool[i].pa - out[k].pa; md = fminf(md, dot(d, d)); }
-      if (md > bd) { bd = md; bi = i; }
-    }
-    if (bi < 0) break;
-    used[bi] = true; out[nc++] = cs.pool[bi];
-  }
-  return nc;
+// point pa of pool entry q
+AG_HD f3 pool_pa(const float* pool, int q) {
+  const float* p = pool + 3 * NARROW_POOL + 3 * q;
+  return f3(p[0], p[1], p[2]);
+}
+// pool entry q as a contact (B-local)
+AG_HD NpOut pool_contact(const float* pool, int q, const FaceRef& F0, const FaceRef& F1) {
+  const bool c1 = (((const int*)pool)[q] & 1) != 0;
+  const float* pb = pool + 6 * NARROW_POOL + 3 * q;
+  NpOut o;
+  o.pa = pool_pa(pool, q); o.pb = f3(pb[0], pb[1], pb[2]);
+  o.n = c1 ? -F1.nf : F0.nf;         // call 0: V is A, normal nf; call 1: V is B, normal -nf
+  o.d = pool[NARROW_POOL + q];
+  return o;
 }
 
-// contacts between colliders ca (A) and cb (B) of env e; results in WORLD coordinates.
-AG_HDN inline int narrow_pair(const SimDev& S, int e, int ca, int cb, float max_dist, bool manifold, NpOut* out) {
+// B-local contact -> world: mapped by (Rw, pw); `flip` swaps the roles of A and B (the half-space is A)
+AG_HD NpOut np_world(const NpOut& c, const m3& Rw, f3 pw, bool flip) {
+  f3 a = mul(Rw, c.pa) + pw, b = mul(Rw, c.pb) + pw, n = mul(Rw, c.n);
+  NpOut o; o.d = c.d;
+  if (!flip) { o.pa = a; o.pb = b; o.n = n; } else { o.pa = b; o.pb = a; o.n = -n; }
+  return o;
+}
+
+// contacts between colliders ca (A) and cb (B) of env e, in WORLD coordinates, handed to emit(k, contact) for k = 0, 1, ...;
+// returns their number.  With `pool` (NARROW_POOL_WORDS words of the thread's scratch) up to 4 contacts of a manifold,
+// without it (nullptr) only the closest-point contact.
+template <class Emit>
+AG_HDN inline int narrow_pair(const SimDev& S, int e, int ca, int cb, float max_dist, float* pool, Emit& emit) {
   const int N = S.N;
   int ta = AG_LDG(S.col_type + ca), tb = AG_LDG(S.col_type + cb);
   float ra = AG_LDG(S.col_radius + ca), rb = AG_LDG(S.col_radius + cb);
@@ -374,16 +442,19 @@ AG_HDN inline int narrow_pair(const SimDev& S, int e, int ca, int cb, float max_
   int pa0 = AG_LDG(S.col_p0 + ca), npA = AG_LDG(S.col_np + ca), pb0 = AG_LDG(S.col_p0 + cb), npB = AG_LDG(S.col_np + cb);
   f3 posA = ld3(S.lpos, ka, N, e), posB = ld3(S.lpos, kb, N, e);
   q4 qA = ld4(S.lquat, ka, N, e), qB = ld4(S.lquat, kb, N, e);
-  CandSel cs; cs.np = 0;
-  int nout;
+  NpOut prim;
+  m3 R, Rw; f3 t, pw; bool flip = false;   // V / A -> local frame; local frame -> world
+  FaceRef F0, F1;                          // face_cands call 0: A's (V's) vertices over B's face; call 1: B's over A's
+  int np_pool = 0;
   if (ta == 3 || tb == 3) {
     if (ta == tb) return 0;
-    bool flip = (ta == 3);                 // half-space is A; compute in the half-space owner's frame
+    flip = (ta == 3);                 // half-space is A; compute in the half-space owner's frame
     // work in the plane owner's local frame: treat owner as "B" of the local computation
     q4 qP = flip ? qA : qB, qV = flip ? qB : qA;
     f3 pP = flip ? posA : posB, pV = flip ? posB : posA;
-    m3 R = mul(transpose(qmat(qP)), qmat(qV));
-    f3 t = qrot_inv(qP, pV - pP);
+    Rw = qmat(qP); pw = pP;
+    R = mul(transpose(Rw), qmat(qV));
+    t = qrot_inv(qP, pV - pP);
     int vv0 = flip ? vb0 : va0, nV = flip ? nB : nA; float rv = flip ? rb : ra;
     f3 pn; float pd; ld_plane(S.planes, flip ? pa0 : pb0, pn, pd);
     int j = 0; float mn = 1e30f;
@@ -392,35 +463,62 @@ AG_HDN inline int narrow_pair(const SimDev& S, int e, int ca, int cb, float max_
     if (d > max_dist) return 0;
     f3 vj = mul(R, tv3(S.verts, vv0 + j)) + t;
     // local result with V playing "A" (normal from plane towards V)
-    cs.prim.pa = vj - pn * rv; cs.prim.pb = vj - pn * (mn - pd); cs.prim.n = pn; cs.prim.d = d;
-    if (manifold && nV > 1) face_cands(S, vv0, nV, rv, true, flip ? pa0 : pb0, 1, 0.f, R, t, pn, d, max_dist * 0.5f, max_dist, cs);
-    nout = select_cands(cs, out);
-    m3 RP = qmat(qP);
-    for (int i = 0; i < nout; i++) {
-      f3 a = mul(RP, out[i].pa) + pP, b = mul(RP, out[i].pb) + pP, n = mul(RP, out[i].n);
-      if (!flip) { out[i].pa = a; out[i].pb = b; out[i].n = n; }
-      else { out[i].pa = b; out[i].pb = a; out[i].n = -n; }
+    prim.pa = vj - pn * rv; prim.pb = vj - pn * (mn - pd); prim.n = pn; prim.d = d;
+    F0 = face_ref(vv0, true, rv, 0.f); F1 = F0;
+    if (pool && nV > 1) face_cands(S, 0, F0, nV, flip ? pa0 : pb0, 1, R, t, pn, d, max_dist * 0.5f, max_dist, pool, np_pool);
+  } else {
+    Rw = qmat(qB); pw = posB;
+    R = mul(transpose(Rw), qmat(qA));
+    t = mulT(Rw, posA - posB);
+    f3 pa, pb, nrm; float dist = 0.f;
+    bool ov = gjk_cores(S.verts, S.vertq, va0, AG_LDG(S.col_g0 + ca), nA, vb0, AG_LDG(S.col_g0 + cb), nB, R, t, pa, pb, nrm, dist);
+    if (ov) { AG_NARROW_STAT(pen_faces, 1); pen_faces(S, va0, nA, pa0, npA, vb0, nB, pb0, npB, R, t, pa, pb, nrm, dist); }
+    float d = dist - ra - rb;
+    if (d > max_dist) return 0;
+    prim.n = nrm; prim.pa = pa - nrm * ra; prim.pb = pb + nrm * rb; prim.d = d;
+    F0 = face_ref(va0, true, ra, rb); F1 = face_ref(vb0, false, rb, ra);
+    if (pool) {
+      if (npB > 0 && nA > 1) face_cands(S, 0, F0, nA, pb0, npB, R, t, nrm, d, max_dist * 0.5f, max_dist, pool, np_pool);
+      if (npA > 0 && nB > 1) face_cands(S, 1, F1, nB, pa0, npA, R, t, -nrm, d, max_dist * 0.5f, max_dist, pool, np_pool);
     }
-    return nout;
   }
-  m3 RB = qmat(qB);
-  m3 R = mul(transpose(RB), qmat(qA));
-  f3 t = mulT(RB, posA - posB);
-  f3 pa, pb, nrm; float dist = 0.f;
-  bool ov = gjk_cores(S.verts, S.vertq, va0, AG_LDG(S.col_g0 + ca), nA, vb0, AG_LDG(S.col_g0 + cb), nB, R, t, pa, pb, nrm, dist);
-  if (ov) pen_faces(S, va0, nA, pa0, npA, vb0, nB, pb0, npB, R, t, pa, pb, nrm, dist);
-  float d = dist - ra - rb;
-  if (d > max_dist) return 0;
-  cs.prim.n = nrm; cs.prim.pa = pa - nrm * ra; cs.prim.pb = pb + nrm * rb; cs.prim.d = d;
-  if (manifold) {
-    if (npB > 0 && nA > 1) face_cands(S, va0, nA, ra, true, pb0, npB, rb, R, t, nrm, d, max_dist * 0.5f, max_dist, cs);
-    if (npA > 0 && nB > 1) face_cands(S, vb0, nB, rb, false, pa0, npA, ra, R, t, -nrm, d, max_dist * 0.5f, max_dist, cs);
+  AG_NARROW_STAT(pool, np_pool);
+  if (np_pool == 0) { emit(0, np_world(prim, Rw, pw, flip)); return 1; }
+  // Manifold selection.  The GJK primary point is arbitrary within a flat contact patch (any point of
+  // two parallel faces is "closest"), so whenever feature candidates exist the manifold is built from
+  // them only: deepest candidate first, then greedily the candidate farthest from the chosen set.
+  const float* pd = pool + NARROW_POOL;
+  float* pmd = pool + 2 * NARROW_POOL;
+  int first = 0;
+  for (int i = 1; i < np_pool; i++) if (pd[i] < pd[first]) first = i;
+  for (int i = 0; i < np_pool; i++) pmd[i] = 1e30f;
+  unsigned used = 1u << first;
+  int nc = 0, cur = first;
+  for (;;) {
+    NpOut c = pool_contact(pool, cur, F0, F1);
+    emit(nc++, np_world(c, Rw, pw, flip));
+    if (nc == 4) break;
+    // pmd[i]: squared distance from candidate i to the nearest chosen contact, brought up to date with the one just chosen
+    // (the same fminf sequence as a minimum over the chosen set in the order they were chosen)
+    int bi = -1; float bd = 1e-8f;
+    for (int i = 0; i < np_pool; i++) {
+      if ((used >> i) & 1u) continue;
+      f3 dv = pool_pa(pool, i) - c.pa;
+      float md = fminf(pmd[i], dot(dv, dv));
+      pmd[i] = md;
+      if (md > bd) { bd = md; bi = i; }
+    }
+    if (bi < 0) break;
+    used |= 1u << bi; cur = bi;
   }
-  nout = select_cands(cs, out);
-  for (int i = 0; i < nout; i++) {
-    out[i].pa = mul(RB, out[i].pa) + posB; out[i].pb = mul(RB, out[i].pb) + posB; out[i].n = mul(RB, out[i].n);
-  }
-  return nout;
+  return nc;
+}
+
+// the closest-point contact of colliders ca and cb within max_dist, in world coordinates
+struct FirstContact { NpOut* c; AG_HD void operator()(int, const NpOut& x) const { *c = x; } };
+AG_HD bool narrow_closest(const SimDev& S, int e, int ca, int cb, float max_dist, NpOut& out) {
+  FirstContact k; k.c = &out;
+  return narrow_pair(S, e, ca, cb, max_dist, nullptr, k) > 0;
 }
 
 AG_HD int ag_atomic_inc(int* p) {
@@ -484,8 +582,24 @@ AG_HDN inline void csort_body(int tid, const SimDev& S, const KP&) {
   S.cand_s[(size_t)rank * N + e] = w;
 }
 
-// K3b: thread = (candidate slot, env): GJK / face fallback / manifold for one collider pair.
-AG_HDN inline void narrow_body(int tid, const SimDev& S, const KP&) {
+// K3b: thread = (candidate slot, env): GJK / face fallback / manifold for one collider pair; `pool` holds NARROW_POOL_WORDS words.
+// Raw contacts land in arrival order in a buffer 4x the contact budget; K4 keeps the `maxc` smallest keys, so which contacts
+// survive an over-budget env does not depend on the arrival order.
+struct RawContacts {
+  const SimDev* S; int e; unsigned pk;
+  AG_HD void operator()(int i, const NpOut& o) const {
+    const int N = S->N;
+    int slot = ag_atomic_inc(S->c_count + e);
+    if (slot >= S->maxraw) return;
+    S->c_key[(size_t)slot * N + e] = pk * 4u + (unsigned)i;
+    float* c = S->c_data + (size_t)slot * AG_CFR * N + e;
+    c[(size_t)CF_PAX * N] = o.pa.x; c[(size_t)CF_PAY * N] = o.pa.y; c[(size_t)CF_PAZ * N] = o.pa.z;
+    c[(size_t)CF_PBX * N] = o.pb.x; c[(size_t)CF_PBY * N] = o.pb.y; c[(size_t)CF_PBZ * N] = o.pb.z;
+    c[(size_t)CF_NX * N] = o.n.x; c[(size_t)CF_NY * N] = o.n.y; c[(size_t)CF_NZ * N] = o.n.z;
+    c[(size_t)CF_DIST * N] = o.d;
+  }
+};
+AG_HDN inline void narrow_body(int tid, const SimDev& S, float* pool) {
   const int N = S.N;
   int e = tid % N, cs = tid / N;
   int ncand = S.cand_count[e]; if (ncand > S.maxcand) ncand = S.maxcand;
@@ -493,20 +607,10 @@ AG_HDN inline void narrow_body(int tid, const SimDev& S, const KP&) {
   unsigned pk = S.cand_s[(size_t)cs * N + e] & 0xffffffu;
   int ca = (int)(pk / (unsigned)S.nc), cb = (int)(pk % (unsigned)S.nc);
   float thr = S.contact_thr * fminf(AG_LDG(S.col_thresh + ca), AG_LDG(S.col_thresh + cb));
-  NpOut out[4];
-  int n = narrow_pair(S, e, ca, cb, thr, true, out);
-  for (int i = 0; i < n; i++) {
-    // raw contacts land in arrival order in a buffer 4x the contact budget; K4 keeps the `maxc` smallest keys,
-    // so which contacts survive an over-budget env does not depend on the arrival order
-    int slot = ag_atomic_inc(S.c_count + e);
-    if (slot >= S.maxraw) continue;
-    S.c_key[(size_t)slot * N + e] = pk * 4u + (unsigned)i;
-    float* c = S.c_data + (size_t)slot * AG_CFR * N + e;
-    c[(size_t)CF_PAX * N] = out[i].pa.x; c[(size_t)CF_PAY * N] = out[i].pa.y; c[(size_t)CF_PAZ * N] = out[i].pa.z;
-    c[(size_t)CF_PBX * N] = out[i].pb.x; c[(size_t)CF_PBY * N] = out[i].pb.y; c[(size_t)CF_PBZ * N] = out[i].pb.z;
-    c[(size_t)CF_NX * N] = out[i].n.x; c[(size_t)CF_NY * N] = out[i].n.y; c[(size_t)CF_NZ * N] = out[i].n.z;
-    c[(size_t)CF_DIST * N] = out[i].d;
-  }
+  RawContacts out; out.S = &S; out.e = e; out.pk = pk;
+  AG_NARROW_STAT(cand, tid);
+  const int n = narrow_pair(S, e, ca, cb, thr, pool, out);
+  AG_NARROW_STAT(done, n);
 }
 
 AG_HD void contact_refs(const SimDev& S, int e, unsigned key, int& refA, int& refB);   // ag_solver.cuh

@@ -96,9 +96,9 @@ AG_HDN inline void closest_body(int e, const SimDev& S, const KP& p) {
         f3 amin = ld3(S.cmin, ca, N, e), amax = ld3(S.cmax, ca, N, e);
         for (int cb = cb0; cb < cb0 + ncb; cb++) {
           if (!aabb_ov(amin, amax, ld3(S.cmin, cb, N, e), ld3(S.cmax, cb, N, e), dist)) continue;
-          NpOut out[4];
-          if (!narrow_pair(S, e, ca, cb, dist, false, out)) continue;
-          if (n < max_pts) write_contact((float*)p.p1 + ((size_t)e * max_pts + n) * 13, la, lb, out[0].pa, out[0].pb, out[0].n, out[0].d, 0.f);
+          NpOut c;
+          if (!narrow_closest(S, e, ca, cb, dist, c)) continue;
+          if (n < max_pts) write_contact((float*)p.p1 + ((size_t)e * max_pts + n) * 13, la, lb, c.pa, c.pb, c.n, c.d, 0.f);
           n++;
         }
       }

@@ -166,8 +166,8 @@ AG_HD bool tool_within(const SimDev& S, int e, int col, int tool_link, float dis
   int c0 = AG_LDG(S.link_col0 + tool_link), ncl = AG_LDG(S.link_ncol + tool_link);
   for (int c = c0; c < c0 + ncl; c++) {
     if (!aabb_ov(pmin, pmax, ld3(S.cmin, c, N, e), ld3(S.cmax, c, N, e), dist)) continue;
-    NpOut out[4];
-    if (narrow_pair(S, e, col, c, dist, false, out)) return true;
+    NpOut out;
+    if (narrow_closest(S, e, col, c, dist, out)) return true;
   }
   return false;
 }

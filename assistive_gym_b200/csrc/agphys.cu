@@ -45,21 +45,27 @@ static int fail(const std::string& m) { g_err = m; return -1; }
   static void name(SimDev S, KP p) { for (int tid = 0; tid < p.n; tid++) body(tid, S, p); }
 #endif
 
-#ifndef AG_CPU_EMU
-#define AG_KERNEL_B(name, body, minblocks)                                      \
-  __global__ void __launch_bounds__(128, minblocks) name(SimDev S, KP p) {      \
-    int tid = blockIdx.x * blockDim.x + threadIdx.x;                            \
-    if (tid < p.n) body(tid, S, p);                                             \
-  }
-#else
-#define AG_KERNEL_B(name, body, minblocks) AG_KERNEL(name, body)
-#endif
 AG_KERNEL(k_fk, fk_body)
 AG_KERNEL(k_aabb, aabb_body)
 AG_KERNEL(k_linkaabb, linkaabb_body)
 AG_KERNEL(k_pairs, pairs_body)
 AG_KERNEL(k_csort, csort_body)
-AG_KERNEL_B(k_narrow, narrow_body, 3)
+// k_narrow: one candidate pair per thread; each thread's manifold pool is its own NARROW_POOL_WORDS-word slice of shared
+// memory (436 B).  64 threads per CTA keep the slices under the 48 KB of static shared memory and give 6 CTAs = 12 warps per
+// SM at the kernel's register count (the register file allows no more).
+#define NARROW_T 64
+#ifndef AG_CPU_EMU
+__global__ void __launch_bounds__(NARROW_T, 6) k_narrow(SimDev S, KP p) {
+  __shared__ float pool[NARROW_T * NARROW_POOL_WORDS];
+  int tid = blockIdx.x * blockDim.x + threadIdx.x;
+  if (tid < p.n) narrow_body(tid, S, pool + threadIdx.x * NARROW_POOL_WORDS);
+}
+#else
+static void k_narrow(SimDev S, KP p) {
+  float pool[NARROW_POOL_WORDS];
+  for (int tid = 0; tid < p.n; tid++) narrow_body(tid, S, pool);
+}
+#endif
 AG_KERNEL(k_sort, sort_body)
 // k_dyn: a CTA is two warps.  Warp 0 runs DYN_T articulated bodies, each lane with its per-dof arrays in its own slice of
 // shared memory (p.i2 = dyn_scratch_words words); warp 1 steps free bodies, grid-stride over all of them, so that their
@@ -896,7 +902,18 @@ static void substep(AgSim* s) {
   KP c = kp0(); c.i0 = Npad;
   LAUNCH(s, k_pairs, (size_t)S.nslice * Npad, c);
   LAUNCH(s, k_csort, (size_t)S.maxcand * N, z);
+#ifndef AG_CPU_EMU
+  {
+    KP kp = z; kp.n = S.maxcand * N;
+    int ps = s->profiling ? prof_slot(s, "k_narrow") : -1;
+    if (ps >= 0) prof_mark(s, ps, true);
+    k_narrow<<<(kp.n + NARROW_T - 1) / NARROW_T, NARROW_T, 0, s->stream>>>(S, kp);
+    if (ps >= 0) prof_mark(s, ps, false);
+    s->launches++;
+  }
+#else
   LAUNCH(s, k_narrow, (size_t)S.maxcand * N, z);
+#endif
   LAUNCH(s, k_sort, (size_t)S.maxraw * N, z);
   {
     KP d = z; d.i0 = S.nart * N; d.i1 = S.nf * N; d.i3 = s->dyn_cap; d.i2 = dyn_scratch_words(d.i3);
