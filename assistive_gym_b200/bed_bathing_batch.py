@@ -74,20 +74,7 @@ def capsule_points(p1, p2, radius, distance_between_points=0.05):
 class BedBathingBatch:
     def __init__(self, controllable_person=False):
         self.controllable_person = bool(controllable_person)
-        b = SceneBuilder()
-        self.builder = b
-        b.set_gravity([0, 0, -9.81])
-        self.plane = b.load_urdf('plane')
-        self.bed = b.load_urdf('bed', base_pos=[-0.1, 0, 0], fixed_base=True)
-        b.change_dynamics(self.bed, -1, lateral_friction=5)                      # bed_bathing.py:117
-        self.humans = {}
-        for gender in ('male', 'female'):
-            hb, info = create_human(b, gender=gender, static=True)
-            for j in range(b.num_joints(hb)):                                    # "static joints" after the settle (bed_bathing.py:133-136)
-                if not (self.controllable_person and j in RIGHT_ARM_JOINTS):  # a controllable arm keeps its mass (human.py:108-112)
-                    b.change_dynamics(hb, j, mass=0)
-            b.set_gravity([0, 0, -1], body=hb)
-            self.humans[gender] = hb
+        b = self._bed_and_persons()
         self.robot = b.load_urdf('sawyer', base_pos=[-1, -1, 0.975], fixed_base=True, self_collision=True)
         for i in range(3, 24):                                                   # sawyer.py:55-61
             for j in range(3, 24):
@@ -111,11 +98,34 @@ class BedBathingBatch:
         self.arm_links = [self.gl(self.robot, j) for j in SAWYER['arm']]
         self.gripper_links = [self.gl(self.robot, j) for j in SAWYER['gripper']]
         self.ee_link = self.gl(self.robot, SAWYER['ee'])
-        self.cloth_link = self.gl(self.tool, WIPER_CLOTH_LINK)
         self.kin = BodyKinematics(sc, self.robot)
-        self.hkin = {g: BodyKinematics(sc, hb) for g, hb in self.humans.items()}
         self.arm_lower = sc['link_lower'][self.arm_links].copy()
         self.arm_upper = sc['link_upper'][self.arm_links].copy()
+        self._person_links()
+
+    def _bed_and_persons(self):
+        """A scene builder holding the plane, the bed and both persons as BedBathing sets them up; the robot and the wiper follow."""
+        b = SceneBuilder()
+        self.builder = b
+        b.set_gravity([0, 0, -9.81])
+        self.plane = b.load_urdf('plane')
+        self.bed = b.load_urdf('bed', base_pos=[-0.1, 0, 0], fixed_base=True)
+        b.change_dynamics(self.bed, -1, lateral_friction=5)                      # bed_bathing.py:117
+        self.humans = {}
+        for gender in ('male', 'female'):
+            hb, info = create_human(b, gender=gender, static=True)
+            for j in range(b.num_joints(hb)):                                    # "static joints" after the settle (bed_bathing.py:133-136)
+                if not (self.controllable_person and j in RIGHT_ARM_JOINTS):  # a controllable arm keeps its mass (human.py:108-112)
+                    b.change_dynamics(hb, j, mass=0)
+            b.set_gravity([0, 0, -1], body=hb)
+            self.humans[gender] = hb
+        return b
+
+    def _person_links(self):
+        """The wiper's cloth link, the persons' kinematics and arm links, and the wiping targets, once the scene is finalised."""
+        sc = self.scene
+        self.cloth_link = self.gl(self.tool, WIPER_CLOTH_LINK)
+        self.hkin = {g: BodyKinematics(sc, hb) for g, hb in self.humans.items()}
         # wiping targets in the upper-arm / forearm link frames (bed_bathing.py:183-184)
         self.targets_local = {}
         for g, (ul, ur, fl, fr) in ARM_DIMS.items():
@@ -244,10 +254,17 @@ class BedBathingBatch:
         return tp, tq
 
     def reset(self, sim, rng, sample=None, base_attempts=6, toc_attempts=50):
+        s = sample or self.sample(sim.n, rng)
+        self.last_sample = s
+        self._reset_person(sim, s)
+        self._reset_sawyer(sim, s, rng, base_attempts, toc_attempts)
+        return s
+
+    def _reset_person(self, sim, s):
+        """Floor friction and both genders in the lying pose with joint noise, lowered onto the mattress; frozen, or simulated when
+        the person is controllable (one gender active per env).  Sets `human_pos` / `human_quat`."""
         n = sim.n
         sc = self.scene
-        s = sample or self.sample(n, rng)
-        self.last_sample = s
         male = s['male'].astype(bool)
         sim.set_link_friction(int(sc['body_link0'][self.plane]), s['plane_friction'])
         # ---- person: lying pose, lowered onto the mattress, frozen
@@ -271,6 +288,10 @@ class BedBathingBatch:
         for g, hb in self.humans.items():
             sim.set_base_pose(hb, hpos, np.tile(lie, (n, 1)))
         self.human_pos, self.human_quat = hpos, np.tile(lie, (n, 1))
+
+    def _reset_sawyer(self, sim, s, rng, base_attempts, toc_attempts):
+        n = sim.n
+        male = s['male'].astype(bool)
         # ---- robot base pose + start joint angles (position_robot_toc's sampling distribution, first feasible draw)
         target = np.array([-0.6, 0.2, 1.0]) + s['ee_offset']
         gq = np.tile(SAWYER['gripper_pos'], (n, 1)).astype(np.float64)
@@ -350,7 +371,6 @@ class BedBathingBatch:
         sim.set_motor(self.arm_links, MOTOR_POSITION, target=arm_q, kp=[0.05] * 7, kd=[1.0] * 7, max_force=[1.0] * 7)
         sim.set_motor(self.gripper_links, MOTOR_POSITION, target=gq, kp=[0.05] * 2, kd=[1.0] * 2, max_force=[500.0] * 2)
         sim.forward_kinematics()
-        return s
 
     def hover_over_forearm(self, sim, s, rng, gap=0.003):
         """Start pose for the dense tool-skin contact workload (SURVEY.md 8(d) config C2): the arm is moved so that the

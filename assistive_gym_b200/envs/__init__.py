@@ -1,4 +1,4 @@
-from .bed_bathing_envs import BedBathingSawyerEnv, BedBathingSawyerHumanEnv  # noqa: F401
+from .bed_bathing_envs import BedBathingPR2Env, BedBathingPR2HumanEnv, BedBathingSawyerEnv, BedBathingSawyerHumanEnv  # noqa: F401
 from .dressing_envs import DressingJacoEnv, DressingJacoHumanEnv, DressingPR2Env, DressingPR2HumanEnv, DressingSawyerEnv, DressingSawyerHumanEnv  # noqa: F401
 from .drinking_envs import DrinkingJacoEnv, DrinkingPR2Env, DrinkingSawyerEnv  # noqa: F401
 from .feeding_envs import FeedingJacoEnv, FeedingJacoHumanEnv, FeedingPR2Env, FeedingPR2HumanEnv, FeedingSawyerEnv, FeedingSawyerHumanEnv  # noqa: F401
@@ -12,7 +12,7 @@ ENV_REGISTRY = {'FeedingJaco-v1': FeedingJacoEnv, 'BedBathingSawyer-v1': BedBath
                 'ScratchItchSawyerHuman-v1': ScratchItchSawyerHumanEnv, 'ScratchItchPR2Human-v1': ScratchItchPR2HumanEnv,
                 'DrinkingSawyer-v1': DrinkingSawyerEnv, 'DrinkingPR2-v1': DrinkingPR2Env,
                 'DressingSawyer-v1': DressingSawyerEnv, 'DressingJaco-v1': DressingJacoEnv, 'DressingSawyerHuman-v1': DressingSawyerHumanEnv,
-                'DressingJacoHuman-v1': DressingJacoHumanEnv}
+                'DressingJacoHuman-v1': DressingJacoHumanEnv, 'BedBathingPR2-v1': BedBathingPR2Env, 'BedBathingPR2Human-v1': BedBathingPR2HumanEnv}
 
 
 def make(env_id, **kw):

@@ -7,7 +7,8 @@ per-call `Agent` API, vectorised over `n_envs` (the per-contact Python loop of `
 bed_bathing.py:41-78, becomes one masked distance test of every tool-cloth contact against every
 remaining wiping target) -- and exists so that tests can show the two paths agree.
 
-With a controllable person (co-optimisation, `BedBathingSawyerHuman-v1`) `step` takes {'robot': a7, 'human': a10} and goes through
+The robot is Sawyer or PR2's left arm, placed by TOC (`bed_bathing_robots_batch.py`).
+With a controllable person (co-optimisation, `BedBathingSawyerHuman-v1`, `BedBathingPR2Human-v1`) `step` takes {'robot': a7, 'human': a10} and goes through
 the per-call path (`step_reference_api`): `take_step` drives the person's right arm, keeps it inside its (per-env scaled) limits
 and the realistic joint limits (human.py:134-152) after every substep, and the wiping targets follow the arm (`update_targets`).
 `step_fused` runs the same co-optimisation step on the device (`ag_coop_step_host`).  Deviations: the person is not settled as a
@@ -23,12 +24,23 @@ MAX_TOOL_CONTACTS = 32
 ARM_LINKS = (R_SHOULDER, R_ELBOW, R_WRIST)
 
 
+def bathing_batch_for(robot, controllable_person):
+    """The batched scene of `robot`'s BedBathing id: Sawyer, or PR2 placed by TOC.  BedBathingJaco is not built: the reference
+    puts a wheelchair-mounted robot on a nightstand (bed_bathing.py:150-154), a model this backend does not have."""
+    from ..bed_bathing_robots_batch import BedBathingPR2Batch
+    from .agents.robot import PR2, Sawyer
+    for cls, batch in ((Sawyer, BedBathingBatch), (PR2, BedBathingPR2Batch)):
+        if type(robot) is cls:
+            return batch(controllable_person=controllable_person)
+    raise KeyError('BedBathing is not built for %s' % type(robot).__name__)
+
+
 class BedBathingEnv(AssistiveEnv):
     def __init__(self, robot, human, n_envs=1, device=0, seed=1001, config=None):
         super().__init__(robot=robot, human=human, task='bed_bathing', n_envs=n_envs, device=device, seed=seed,
                          obs_robot_len=(17 + len(robot.controllable_joint_indices) - (len(robot.wheel_joint_indices) if robot.mobile else 0)),
                          obs_human_len=(18 + len(human.controllable_joint_indices)))
-        self._bb = BedBathingBatch(controllable_person=human.controllable)
+        self._bb = bathing_batch_for(robot, human.controllable)
         self._cfg = config or capi.default_config()
         self._sim_lib = None
 

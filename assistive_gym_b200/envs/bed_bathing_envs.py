@@ -1,5 +1,5 @@
 from .agents.human import Human
-from .agents.robot import Sawyer
+from .agents.robot import PR2, Sawyer
 from .bed_bathing import BedBathingEnv
 
 robot_arm = 'left'
@@ -22,4 +22,20 @@ class BedBathingSawyerHumanEnv(BedBathingEnv):
 
     def __init__(self, n_envs=1, device=0, seed=1001, config=None):
         super().__init__(robot=Sawyer(robot_arm), human=Human(human_controllable_joint_indices, controllable=True),
+                         n_envs=n_envs, device=device, seed=seed, config=config)
+
+
+class BedBathingPR2Env(BedBathingEnv):
+    """`assistive_gym:BedBathingPR2-v1` (reference envs/bed_bathing_envs.py:15-17): PR2's left arm, its base placed by TOC."""
+
+    def __init__(self, n_envs=1, device=0, seed=1001, config=None):
+        super().__init__(robot=PR2(robot_arm), human=Human(human_controllable_joint_indices, controllable=False),
+                         n_envs=n_envs, device=device, seed=seed, config=config)
+
+
+class BedBathingPR2HumanEnv(BedBathingEnv):
+    """`assistive_gym:BedBathingPR2Human-v1` (reference envs/bed_bathing_envs.py:39-41): as BedBathingSawyerHuman-v1, with PR2's left arm."""
+
+    def __init__(self, n_envs=1, device=0, seed=1001, config=None):
+        super().__init__(robot=PR2(robot_arm), human=Human(human_controllable_joint_indices, controllable=True),
                          n_envs=n_envs, device=device, seed=seed, config=config)
