@@ -19,7 +19,7 @@ Differences forced by lock-step batching or by what the backend does not simulat
 With `controllable_person=True` (BedBathingSawyerHuman-v1) the person's right arm is a second agent: its ten joints keep their
 mass (`setup_joints(use_static_joints=True, reactive_force=None)` with a controllable person, human.py:104-127), the active
 gender is simulated instead of frozen, and the impairment is drawn with 'no_tremor' (as FeedingJacoHuman-v1 does, feeding.py:59).
-`tremor` is not built for a controllable person: the co-optimisation kernels keep no per-env rest angles.  `weakness` is drawn but
+`tremor` is drawn for a controllable person only when the env is given `human_impairment` (`start_coop` arms it).  `weakness` is drawn but
 does not act: the task sets no reactive force, and take_step's control() drives the arm with motor_forces 1.0.  The wiping targets
 then follow the arm (update_targets, bed_bathing.py:190-203), from their link frames (`target_frames`).
 """
@@ -177,6 +177,15 @@ class BedBathingBatch:
         P = coop_params(self.scene, self.humans, 2, RIGHT_ARM_JOINTS, 0.05)
         w = pack_mlp(P, load_model(), R_ARM_LIMIT_JOINTS, -1.0)
         sim.coop_init(P, limit_scale=s.get('limit_scale'), mlp=w)
+        imp = s.get('impairment')
+        if imp is not None and np.any(imp == 3):       # a tremor person (human_impairment given to the env)
+            sim.coop_set_tremor(imp == 3, self.coop_tremor_target(s), s['tremors'])
+
+    def coop_tremor_target(self, s):
+        """target_joint_angles [n, 10] of a controllable tremor person (human.py:123): the right arm of the lying pose"""
+        male = s['male'].astype(bool)
+        poses = self.human_pose(s)
+        return np.where(male[:, None], poses['male'][1][:, RIGHT_ARM_JOINTS], poses['female'][1][:, RIGHT_ARM_JOINTS])
 
     # ------------------------------------------------------------------ batched reset
     def sample(self, n, rng):

@@ -271,6 +271,7 @@ def load_library(path=None):
     lib.ag_coop_step_dev.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     lib.ag_coop_step_host.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     lib.ag_coop_classify.argtypes = [vp, ci, vp, vp]
+    lib.ag_coop_set_tremor.argtypes = [vp, vp, vp, vp]
     lib.ag_render.argtypes = [vp, C.POINTER(AgCamera), ci, vp, vp, vp]
     lib.ag_ik_solve.argtypes = [vp, ci, vp, ci, vp, vp, ci, ci, C.c_float, C.c_uint64, vp, vp, vp]
     lib.ag_state_size.restype = C.c_size_t
@@ -302,6 +303,6 @@ EXPORTED_SYMBOLS = [
     'ag_cloth_init', 'ag_cloth_set_state', 'ag_cloth_get_state', 'ag_cloth_set_anchor', 'ag_cloth_anchor_follow', 'ag_cloth_set_gravity',
     'ag_cloth_get_contacts', 'ag_cloth_device_state', 'ag_scratch_init', 'ag_scratch_step_dev', 'ag_scratch_step_host', 'ag_render', 'ag_set_body_gravity', 'ag_get_link_aabb', 'ag_dressing_init', 'ag_dressing_reset_episode', 'ag_dressing_set_tremor', 'ag_set_motor_force_scale', 'ag_dressing_step_dev', 'ag_dressing_step_host',
     'ag_overflow_count', 'ag_get_solver_stats', 'ag_get_pgs_cycles', 'ag_get_pgs_trips', 'ag_get_pgs_occupancy', 'ag_profile_enable', 'ag_profile_get',
-    'ag_coop_init', 'ag_coop_step_dev', 'ag_coop_step_host', 'ag_coop_classify', 'ag_bathing_set_target_frames',
+    'ag_coop_init', 'ag_coop_set_tremor', 'ag_coop_step_dev', 'ag_coop_step_host', 'ag_coop_classify', 'ag_bathing_set_target_frames',
     'ag_drinking_init', 'ag_drinking_step_dev', 'ag_drinking_step_host', 'ag_drinking_get_state',
 ]

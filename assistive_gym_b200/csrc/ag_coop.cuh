@@ -4,7 +4,9 @@
 // Reference semantics restated here:
 //   coop_pre      AssistiveEnv.take_step for the Human agent (envs/env.py:174-222): the human slice of the action, clipped and
 //                 x 0.05 (the Robot-only action_multiplier does not apply), accumulated frame_skip times inside the person's
-//                 controllable limits (scaled per env by Human.set_limit_scale) -> motor targets
+//                 controllable limits (scaled per env by Human.set_limit_scale) -> motor targets; for a tremor person
+//                 (ag_coop_set_tremor) accumulated into the env's target_joint_angles instead, the motors driven to
+//                 target +- amplitude (env.py:212-215).  The task's own tremor (k_feed_pre / k_dress_pre) is off in this step.
 //   coop_limits   after every stepSimulation (env.py:223-231): Human.enforce_joint_limits over every joint of the person, then
 //                 Human.enforce_realistic_joint_limits (agents/human.py:134-152): the joint-limit MLP classifies the arm pose,
 //                 an unreachable pose is replaced by the env's last reachable one
@@ -37,6 +39,10 @@ struct CoopDev {
   double* limit_scale;      // [N]
   float* prev_pose;         // [4][N] last reachable shoulder x/y/z + elbow; NaN = none yet (human.py:68 `None`)
   const float* mlp;         // [AG_MLP_FLOATS], packed as in agphys.h
+  const int* iteration;     // the task's per-env step counter, advanced by the task's pre kernel before k_coop_pre runs
+  int* tremor_on;           // [N] the person's impairment is 'tremor' (human.py:80-92); all 0 unless ag_coop_set_tremor
+  double* tremor_target;    // [AG_COOP_MAXC][N] target_joint_angles (human.py:123), accumulated by the action (env.py:214)
+  float* tremor_amp;        // [AG_COOP_MAXC][N] the tremor amplitudes (human.py:87-92)
 };
 
 // The 4-64-64-64-1 classifier: tanh hidden layers, sigmoid output.  `h` is the caller's scratch of 2 x 64 floats with element
@@ -87,7 +93,9 @@ AG_HD void coop_mlp_input(const float ang[4], double sign, float x[4]) {
   x[3] = (float)py_mod(-(double)ang[3] + two_pi, two_pi);
 }
 
-// p0 = action [N][7 + n_ctrl] (env-major), p1 = CoopDev*
+// p0 = action [N][7 + n_ctrl] (env-major), p1 = CoopDev*.  A tremor person (env.py:205-215): the limit checks and the zeroing of
+// the action run against the angles of the previous pass, the action accumulates into the env's target, and the angles become
+// target + amplitude, its sign flipping with the task's step counter (already advanced for this step).
 AG_HDN inline void coop_pre_body(int e, const SimDev& S, const KP& p) {
   const int N = S.N;
   const CoopDev& C = *(const CoopDev*)p.p1;
@@ -95,15 +103,28 @@ AG_HDN inline void coop_pre_body(int e, const SimDev& S, const KP& p) {
   const float* act = (const float*)p.p0 + (size_t)e * (7 + P.n_ctrl) + 7;
   const int* links = C.male[e] ? P.joint_links_m : P.joint_links_f;
   const double sc = C.limit_scale[e];
+  const bool tremor = C.tremor_on[e] != 0;
   for (int c = 0; c < P.n_ctrl; c++) {
     const int j = P.ctrl[c], k = links[j];
     double a = fmin(fmax((double)act[c], -1.0), 1.0) * 0.05;
     double q = ld1(S.jq, k, N, e);
     const double lo = (double)P.joint_lower[j] * sc, hi = (double)P.joint_upper[j] * sc;
-    for (int s = 0; s < C.frame_skip; s++) {
-      if (q + a < lo) { a = 0.0; q = lo; }
-      if (q + a > hi) { a = 0.0; q = hi; }
-      q += a;
+    if (!tremor) {
+      for (int s = 0; s < C.frame_skip; s++) {
+        if (q + a < lo) { a = 0.0; q = lo; }
+        if (q + a > hi) { a = 0.0; q = hi; }
+        q += a;
+      }
+    } else {
+      const double wobble = (double)C.tremor_amp[(size_t)c * N + e] * (C.iteration[e] % 2 == 0 ? 1.0 : -1.0);
+      double t = C.tremor_target[(size_t)c * N + e];
+      for (int s = 0; s < C.frame_skip; s++) {
+        if (q + a < lo) { a = 0.0; q = lo; }
+        if (q + a > hi) { a = 0.0; q = hi; }
+        t += a;
+        q = t + wobble;
+      }
+      C.tremor_target[(size_t)c * N + e] = t;
     }
     st1(S.motor_target, k, N, e, (float)q);
   }

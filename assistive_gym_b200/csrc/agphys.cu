@@ -8,6 +8,7 @@
 #include <string>
 #include <vector>
 #include <algorithm>
+#include <cmath>
 #include "../../include/agphys.h"
 #include "ag_device.cuh"
 #include "ag_solver.cuh"
@@ -271,6 +272,9 @@ struct AgSim {
   size_t render_pix; int render_n; int* d_render_ids; unsigned char* d_render_rgba; float* d_render_depth; void* d_render_dev;
   // co-optimisation (the person's half; the robot's half is the task's state above)
   CoopDev CO; CoopDev* CO_dev; bool coop;
+  // some env's tremor is on: the person's (ag_coop_set_tremor), the single-agent Feeding / Dressing person's (ag_*_set_tremor).
+  // k_coop_pre and the task's pre kernel would both drive the person's motors, so the two are never on together.
+  bool coop_tremor, feed_tremor, dress_tremor;
   // the fused-step entry points (Task, then IO_COOP); CUDA-graph replay of their steps
   StepIO io[6];
   bool use_graph; int graph_failures;
@@ -1204,6 +1208,19 @@ static int* task_male(const AgSim* s, Task task) {
   }
   return nullptr;
 }
+static int* task_iteration(const AgSim* s, Task task) {
+  switch (task) {
+    case TASK_FEEDING: return s->F.iteration;
+    case TASK_SCRATCH: return s->SD.iteration;
+    case TASK_BATHING: return s->B.iteration;
+    case TASK_DRESSING: return s->DP.D.iteration;
+    case TASK_DRINKING: return s->DK.iteration;
+  }
+  return nullptr;
+}
+static bool task_tremor(const AgSim* s, Task task) {
+  return (task == TASK_FEEDING && s->feed_tremor) || (task == TASK_DRESSING && s->dress_tremor);
+}
 
 // An entry point's buffers, allocated at its first init: device buffers, then pinned staging for the host-buffer step.
 static int io_alloc(AgSim* s, StepIO& io, int act_w, int obs_w, int obs_h_w) {
@@ -1343,6 +1360,8 @@ static int step_check(const AgSim* s, Task task, bool coop) {
   if (!task_ready(s, task)) return fail(std::string(TASK_INIT[task]) + " not called");
   if (coop && task == TASK_BATHING && !s->bath_frames) return fail("ag_coop_step: call ag_bathing_set_target_frames after ag_bathing_init");
   if (task == TASK_DRESSING && s->cloth_sub != 0) return fail("fused dressing step: a stepSimulation is half done (ag_step with a partial substep count?)");
+  if (coop && s->coop_tremor && task_tremor(s, task))
+    return fail("ag_coop_step: the task's own tremor was switched on after ag_coop_set_tremor; only one of them may drive the person");
   return 0;
 }
 static StepIO& step_io(AgSim* s, Task task, bool coop) { return s->io[coop ? IO_COOP : task]; }
@@ -1618,6 +1637,7 @@ int ag_dressing_init(AgSim* s, const AgDressingParams* p, const int32_t* gender_
     if (io_alloc(s, s->io[TASK_DRESSING], 7, ROBOT_OBS_W[TASK_DRESSING], 0)) return -1;
   }
   else if (dev_zero(s, D.tremor_on, sizeof(int) * N)) return -1;
+  s->dress_tremor = false;
   for (int j = 0; j < 10; j++) if (p->human_arm_m[j] < 0 || p->human_arm_m[j] >= s->nl || p->human_arm_f[j] < 0 || p->human_arm_f[j] >= s->nl) return fail("ag_dressing_init: bad human arm link");
   s->DP.C = s->C_dev;
   if (h2d(s, D.male, gender_is_male, sizeof(int) * N)) return -1;
@@ -1635,6 +1655,7 @@ int ag_dressing_set_tremor(AgSim* s, const int32_t* on, const float* rest, const
     for (int j = 0; j < 10; j++) { r[(size_t)j * N + e] = rest ? rest[(size_t)e * 10 + j] : 0.f; a[(size_t)j * N + e] = amplitude ? amplitude[(size_t)e * 10 + j] : 0.f; }
   }
   if (h2d(s, s->DP.D.tremor_on, o.data(), sizeof(int) * N) || h2d(s, s->DP.D.tremor_rest, r.data(), sizeof(float) * 10 * N)) return -1;
+  s->dress_tremor = std::any_of(o.begin(), o.end(), [](int v) { return v != 0; });
   return h2d(s, s->DP.D.tremor_amp, a.data(), sizeof(float) * 10 * N);
 }
 int ag_dressing_step_dev(AgSim* s, const float* action_dev, float* obs_dev, float* reward_dev, float* done_dev, float* info_dev) {
@@ -1789,6 +1810,7 @@ int ag_feeding_init(AgSim* s, const AgFeedingParams* p, const int32_t* gender_is
   } else {
     if (dev_zero(s, F.tremor_on, sizeof(int) * N) || dev_zero(s, F.rng, sizeof(unsigned long long) * N)) return -1;
   }
+  s->feed_tremor = false;
   if (h2d(s, F.male, gender_is_male, sizeof(int) * N)) return -1;
   if (!s->F_dev || h2d(s, s->F_dev, &s->F, sizeof(FeedDev))) return fail("FeedDev upload failed");
   s->feeding = true;
@@ -1804,6 +1826,7 @@ int ag_feeding_set_tremor(AgSim* s, const int32_t* on, const float* rest, const 
     for (int j = 0; j < 4; j++) { r[(size_t)j * N + e] = rest ? rest[(size_t)e * 4 + j] : 0.f; a[(size_t)j * N + e] = amplitude ? amplitude[(size_t)e * 4 + j] : 0.f; }
   }
   if (h2d(s, s->F.tremor_on, o.data(), sizeof(int) * N)) return -1;
+  s->feed_tremor = std::any_of(o.begin(), o.end(), [](int v) { return v != 0; });
   if (h2d(s, s->F.tremor_rest, r.data(), sizeof(float) * 4 * N)) return -1;
   return h2d(s, s->F.tremor_amp, a.data(), sizeof(float) * 4 * N);
 }
@@ -1949,8 +1972,10 @@ int ag_coop_init(AgSim* s, const AgCoopParams* p, const double* limit_scale, con
   if (!s->coop) {             // buffers are allocated once; a later init (episode reset) only refreshes their contents
     C.limit_scale = dalloc<double>(s, N); C.prev_pose = dalloc<float>(s, (size_t)4 * N);
     C.mlp = dalloc<float>(s, AG_MLP_FLOATS);
+    C.tremor_on = dalloc<int>(s, N);
+    C.tremor_target = dalloc<double>(s, (size_t)AG_COOP_MAXC * N); C.tremor_amp = dalloc<float>(s, (size_t)AG_COOP_MAXC * N);
     s->CO_dev = dalloc<CoopDev>(s, 1);
-    if (!s->CO_dev) return fail("device allocation failed");
+    if (!s->CO_dev || !C.tremor_on || !C.tremor_target || !C.tremor_amp) return fail("device allocation failed");
     // room for every task's widths; each init sets its own task's below
     if (io_alloc(s, io, 7 + AG_COOP_MAXC, *std::max_element(ROBOT_OBS_W, ROBOT_OBS_W + 4), *std::max_element(HUMAN_OBS_W, HUMAN_OBS_W + 4))) return -1;
 #ifndef AG_CPU_EMU
@@ -1962,8 +1987,11 @@ int ag_coop_init(AgSim* s, const AgCoopParams* p, const double* limit_scale, con
   C.frame_skip = task_frame_skip(s, task);
   C.male = task_male(s, task);
   C.mlp_on = mlp != nullptr;
+  C.iteration = task_iteration(s, task);
   std::vector<float> none((size_t)4 * N, nanf(""));
   if (h2d(s, C.limit_scale, sc.data(), sizeof(double) * N) || h2d(s, C.prev_pose, none.data(), sizeof(float) * 4 * N)) return -1;
+  if (dev_zero(s, C.tremor_on, sizeof(int) * N)) return -1;       // a re-armed batch starts without the last episode's tremor
+  s->coop_tremor = false;
   if (mlp && h2d(s, (void*)C.mlp, mlp, sizeof(float) * AG_MLP_FLOATS)) return -1;
   if (h2d(s, s->CO_dev, &C, sizeof(CoopDev))) return -1;
   // take_step's control() re-issues the person's gains / forces every step; the first step would set these anyway
@@ -1976,6 +2004,28 @@ int ag_coop_init(AgSim* s, const AgCoopParams* p, const double* limit_scale, con
   if (ag_set_motor_host(s, (int)links.size(), links.data(), 1, nullptr, kp.data(), kd.data(), mf.data())) return -1;
   io.act_w = 7 + p->n_ctrl; io.obs_w = ROBOT_OBS_W[task]; io.obs_h_w = HUMAN_OBS_W[task];
   s->coop = true;
+  return 0;
+}
+int ag_coop_set_tremor(AgSim* s, const int32_t* on, const double* target, const float* amplitude) {
+  DevGuard guard__(s->device);
+  if (!s->coop) return fail("ag_coop_set_tremor: call ag_coop_init first");
+  const int N = s->S.N, k = s->CO.P.n_ctrl;
+  std::vector<int> o(N, 0);
+  if (on) for (int e = 0; e < N; e++) o[e] = on[e] != 0;
+  const bool any = std::any_of(o.begin(), o.end(), [](int v) { return v != 0; });
+  if (any && (!target || !amplitude)) return fail("ag_coop_set_tremor: bad arguments (target and amplitude are needed with a tremor env)");
+  if (any && task_tremor(s, (Task)s->CO.P.task))
+    return fail("ag_coop_set_tremor: the task's own tremor (ag_feeding_set_tremor / ag_dressing_set_tremor) is on; switch it off: in the "
+                "co-optimisation step k_coop_pre drives the person's controllable joints");
+  std::vector<double> t((size_t)k * N, 0.0); std::vector<float> a((size_t)k * N, 0.f);
+  for (int e = 0; e < N; e++)
+    if (o[e]) for (int c = 0; c < k; c++) {
+      t[(size_t)c * N + e] = target[(size_t)e * k + c]; a[(size_t)c * N + e] = amplitude[(size_t)e * k + c];
+      if (!std::isfinite(t[(size_t)c * N + e]) || !std::isfinite(a[(size_t)c * N + e])) return fail("ag_coop_set_tremor: target and amplitude must be finite");
+    }
+  if (h2d(s, s->CO.tremor_on, o.data(), sizeof(int) * N) || h2d(s, s->CO.tremor_target, t.data(), sizeof(double) * k * N) ||
+      h2d(s, s->CO.tremor_amp, a.data(), sizeof(float) * k * N)) return -1;
+  s->coop_tremor = any;
   return 0;
 }
 int ag_coop_step_dev(AgSim* s, const float* action_dev, float* obs_robot_dev, float* obs_human_dev, float* reward_dev, float* done_dev, float* info_dev) {

@@ -314,10 +314,18 @@ class DressingBatch(TocPlacement):
         P = coop_params(self.scene, self.humans, 3, LEFT_ARM_JOINTS, 0.01)
         w = pack_mlp(P, load_model(), L_ARM_LIMIT_JOINTS, 1.0)
         sim.coop_init(P, limit_scale=s.get('limit_scale'), mlp=w)
+        imp = s.get('impairment')
+        if imp is not None and np.any(imp == 3):       # a tremor person (human_impairment given to the env)
+            sim.coop_set_tremor(imp == 3, self.coop_tremor_target(s), s['tremors'])
+
+    def coop_tremor_target(self, s):
+        """target_joint_angles [n, 10] of a controllable tremor person (human.py:123): the left arm's preset, before the gown
+        settles"""
+        return self.human_rest
 
     def start_fused(self, sim, sample=None):
         s = sample or self.last_sample
         sim.dressing_init(self.dressing_params(), s['male'])
         imp = s.get('impairment')
-        if imp is not None and np.any(imp == 3):
+        if imp is not None and np.any(imp == 3) and not self.controllable_person:     # a controllable person's: start_coop
             sim.dressing_set_tremor((imp == 3).astype(np.int32), self.human_rest, s['tremors'])

@@ -12,7 +12,7 @@ With a controllable person (co-optimisation, `BedBathingSawyerHuman-v1`, `BedBat
 the per-call path (`step_reference_api`): `take_step` drives the person's right arm, keeps it inside its (per-env scaled) limits
 and the realistic joint limits (human.py:134-152) after every substep, and the wiping targets follow the arm (`update_targets`).
 `step_fused` runs the same co-optimisation step on the device (`ag_coop_step_host`).  Deviations: the person is not settled as a
-ragdoll at reset (it is lowered onto the mattress, as for the static person), and `tremor` is not drawn for it."""
+ragdoll at reset (it is lowered onto the mattress, as for the static person), and `tremor` is drawn for it only with `human_impairment` (AssistiveEnv)."""
 import numpy as np
 
 from .. import capi
@@ -36,8 +36,8 @@ def bathing_batch_for(robot, controllable_person):
 
 
 class BedBathingEnv(AssistiveEnv):
-    def __init__(self, robot, human, n_envs=1, device=0, seed=1001, config=None):
-        super().__init__(robot=robot, human=human, task='bed_bathing', n_envs=n_envs, device=device, seed=seed,
+    def __init__(self, robot, human, n_envs=1, device=0, seed=1001, config=None, human_impairment=None):
+        super().__init__(robot=robot, human=human, task='bed_bathing', n_envs=n_envs, device=device, seed=seed, human_impairment=human_impairment,
                          obs_robot_len=(17 + len(robot.controllable_joint_indices) - (len(robot.wheel_joint_indices) if robot.mobile else 0)),
                          obs_human_len=(18 + len(human.controllable_joint_indices)))
         self._bb = bathing_batch_for(robot, human.controllable)
@@ -107,7 +107,7 @@ class BedBathingEnv(AssistiveEnv):
             self._attach(bb, bb.bed, BatchSim)
         rng = np.random.default_rng(self.np_random.randint(0, 2 ** 31 - 1))
         self.agents = [self.robot]
-        s = bb.reset(self.id, rng)
+        s = bb.reset(self.id, rng, sample=self._person_sample(bb, rng))
         self.male = s['male'].astype(bool)
         self.human.gender = 'male' if self.male[0] else 'female'
         if self.human.controllable:
@@ -115,6 +115,8 @@ class BedBathingEnv(AssistiveEnv):
             for h in self.humans.values():
                 h.enforce_joint_limits(h.controllable_joint_indices)              # the start pose is clipped to them (human.py:115)
             self.id.forward_kinematics()
+            if self.human_impairment_coop is not None:
+                self._person_tremor(s, bb.coop_tremor_target(s))
         self.generate_targets(s)
         if self.human.controllable:
             bb.start_coop(self.id, s)

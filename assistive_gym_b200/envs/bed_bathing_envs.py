@@ -20,9 +20,9 @@ class BedBathingSawyerHumanEnv(BedBathingEnv):
     learn.py:41-59).  The person's right arm is driven by its action and kept inside the realistic joint limits; the wiping targets
     follow the arm.  Per-call API path; `step_fused` is the same step on the device."""
 
-    def __init__(self, n_envs=1, device=0, seed=1001, config=None):
+    def __init__(self, n_envs=1, device=0, seed=1001, config=None, human_impairment=None):
         super().__init__(robot=Sawyer(robot_arm), human=Human(human_controllable_joint_indices, controllable=True),
-                         n_envs=n_envs, device=device, seed=seed, config=config)
+                         n_envs=n_envs, device=device, seed=seed, config=config, human_impairment=human_impairment)
 
 
 class BedBathingPR2Env(BedBathingEnv):
@@ -36,6 +36,6 @@ class BedBathingPR2Env(BedBathingEnv):
 class BedBathingPR2HumanEnv(BedBathingEnv):
     """`assistive_gym:BedBathingPR2Human-v1` (reference envs/bed_bathing_envs.py:39-41): as BedBathingSawyerHuman-v1, with PR2's left arm."""
 
-    def __init__(self, n_envs=1, device=0, seed=1001, config=None):
+    def __init__(self, n_envs=1, device=0, seed=1001, config=None, human_impairment=None):
         super().__init__(robot=PR2(robot_arm), human=Human(human_controllable_joint_indices, controllable=True),
-                         n_envs=n_envs, device=device, seed=seed, config=config)
+                         n_envs=n_envs, device=device, seed=seed, config=config, human_impairment=human_impairment)

@@ -10,7 +10,7 @@ With a controllable person (co-optimisation, `Dressing{PR2,Sawyer,Jaco}Human-v1`
 per-call path (`step_reference_api`): `take_step` drives the person's left arm and, after every stepSimulation, keeps it inside its
 (per-env scaled) limits and the realistic joint limits (human.py:134-152), then moves the gown's anchor to the end effector
 (`update_targets`); the observation, the sleeve-on-arm reward and the cloth forces are computed on the host.  `step_fused` runs
-the same co-optimisation step on the device (`ag_coop_step_host`).  `tremor` is not drawn for a controllable person."""
+the same co-optimisation step on the device (`ag_coop_step_host`).  `tremor` is drawn for a controllable person only with `human_impairment` (AssistiveEnv)."""
 import numpy as np
 
 from .. import capi
@@ -32,8 +32,8 @@ def dressing_batch_for(robot, controllable_person=False):
 
 
 class DressingEnv(AssistiveEnv):
-    def __init__(self, robot, human, n_envs=1, device=0, seed=1001, config=None, toc_attempts=50):
-        super().__init__(robot=robot, human=human, task='dressing', n_envs=n_envs, device=device, seed=seed,
+    def __init__(self, robot, human, n_envs=1, device=0, seed=1001, config=None, toc_attempts=50, human_impairment=None):
+        super().__init__(robot=robot, human=human, task='dressing', n_envs=n_envs, device=device, seed=seed, human_impairment=human_impairment,
                          obs_robot_len=(17 + len(robot.controllable_joint_indices) - (len(robot.wheel_joint_indices) if robot.mobile else 0)),
                          obs_human_len=(18 + len(human.controllable_joint_indices)))
         self._db = dressing_batch_for(robot, controllable_person=human.controllable)
@@ -112,7 +112,7 @@ class DressingEnv(AssistiveEnv):
         rng = np.random.default_rng(self.np_random.randint(0, 2 ** 31 - 1))
         self.agents = [self.robot]
         self.robot.motor_gains = self.human.motor_gains = 0.01             # dressing.py:117
-        s = db.reset(self.id, rng, attempts=self._toc_attempts)
+        s = db.reset(self.id, rng, sample=self._person_sample(db, rng), attempts=self._toc_attempts)
         self.male = s['male'].astype(bool)
         self.human.gender = 'male' if self.male[0] else 'female'
         self.start_ee_pos = db.start_ee_pos
@@ -120,6 +120,8 @@ class DressingEnv(AssistiveEnv):
             self._controllable_person(s['limit_scale'])
             for h in self.humans.values():
                 h.motor_gains, h.motor_forces = 0.01, 1.0                         # dressing.py:121; Human.motor_forces
+            if self.human_impairment_coop is not None:
+                self._person_tremor(s, db.coop_tremor_target(s))
         db.start_fused(self.id, s)
         if self.human.controllable:
             db.start_coop(self.id, s)

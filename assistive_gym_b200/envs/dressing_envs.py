@@ -20,9 +20,9 @@ class DressingPR2HumanEnv(DressingEnv):
     learn.py:41-59).  The person's left arm is driven by its action and kept inside the realistic joint limits while the robot
     pulls the gown's sleeve onto it.  Per-call API path; `step_fused` is the same step on the device."""
 
-    def __init__(self, n_envs=1, device=0, seed=1001, config=None, toc_attempts=50):
+    def __init__(self, n_envs=1, device=0, seed=1001, config=None, toc_attempts=50, human_impairment=None):
         super().__init__(robot=PR2(robot_arm), human=Human(human_controllable_joint_indices, controllable=True),
-                         n_envs=n_envs, device=device, seed=seed, config=config, toc_attempts=toc_attempts)
+                         n_envs=n_envs, device=device, seed=seed, config=config, toc_attempts=toc_attempts, human_impairment=human_impairment)
 
 
 class DressingSawyerEnv(DressingEnv):
@@ -44,14 +44,14 @@ class DressingJacoEnv(DressingEnv):
 class DressingSawyerHumanEnv(DressingEnv):
     """`assistive_gym:DressingSawyerHuman-v1` (reference envs/dressing_envs.py:49-52): DressingPR2Human-v1's two agents with Sawyer."""
 
-    def __init__(self, n_envs=1, device=0, seed=1001, config=None, toc_attempts=50):
+    def __init__(self, n_envs=1, device=0, seed=1001, config=None, toc_attempts=50, human_impairment=None):
         super().__init__(robot=Sawyer(robot_arm), human=Human(human_controllable_joint_indices, controllable=True),
-                         n_envs=n_envs, device=device, seed=seed, config=config, toc_attempts=toc_attempts)
+                         n_envs=n_envs, device=device, seed=seed, config=config, toc_attempts=toc_attempts, human_impairment=human_impairment)
 
 
 class DressingJacoHumanEnv(DressingEnv):
     """`assistive_gym:DressingJacoHuman-v1` (reference envs/dressing_envs.py:54-57): DressingPR2Human-v1's two agents with Jaco."""
 
-    def __init__(self, n_envs=1, device=0, seed=1001, config=None, toc_attempts=50):
+    def __init__(self, n_envs=1, device=0, seed=1001, config=None, toc_attempts=50, human_impairment=None):
         super().__init__(robot=Jaco(robot_arm), human=Human(human_controllable_joint_indices, controllable=True),
-                         n_envs=n_envs, device=device, seed=seed, config=config, toc_attempts=toc_attempts)
+                         n_envs=n_envs, device=device, seed=seed, config=config, toc_attempts=toc_attempts, human_impairment=human_impairment)

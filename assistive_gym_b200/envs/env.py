@@ -63,10 +63,20 @@ radius_scale = 1.0
 height_scale = 1.0
 """
 
+IMPAIRMENTS = ('none', 'limits', 'weakness', 'tremor')      # human.py:80-81, in the order of the reference's np_random.choice
+
 
 class AssistiveEnv(gym.Env):
     def __init__(self, robot=None, human=None, task='', obs_robot_len=0, obs_human_len=0, time_step=0.02, frame_skip=5,
-                 render=False, gravity=-9.81, seed=1001, n_envs=1, device=0):
+                 render=False, gravity=-9.81, seed=1001, n_envs=1, device=0, human_impairment=None):
+        if human_impairment is not None:
+            if not (human is not None and human.controllable):
+                raise ValueError('human_impairment selects the impairment of a controllable person (the co-optimisation ids)')
+            if human_impairment not in ('random',) + IMPAIRMENTS:
+                raise ValueError("human_impairment must be None, 'random' or one of %s" % (IMPAIRMENTS,))
+        # None: the person's impairment as each task draws it without the keyword (never 'tremor'); 'random': the reference's
+        # four-way draw (human.py:80-81); a name forces that impairment in every env
+        self.human_impairment_coop = human_impairment
         self.task = task
         self.time_step, self.frame_skip, self.gravity = time_step, frame_skip, gravity
         self.n_envs, self.device = int(n_envs), device
@@ -189,11 +199,22 @@ class AssistiveEnv(gym.Env):
                 action *= agent.action_multiplier
             q = np.atleast_2d(agent.get_joint_angles(agent.controllable_joint_indices)).copy()
             lo, hi = agent.controllable_joint_lower_limits, agent.controllable_joint_upper_limits
+            # a controllable tremor person (env.py:205-215): per env, the action accumulates into target_joint_angles and the
+            # joints are driven to target + tremors x (+-1); the limit checks run against the previous pass's angles
+            trem = agent.tremor_mask[:, None] if isinstance(agent, Human) and agent.impairment == 'tremor' else None
+            if trem is not None:
+                target, wobble = agent.target_joint_angles, agent.tremors * (1.0 if self.iteration % 2 == 0 else -1.0)
             for _ in range(self.frame_skip):
                 below, above = q + action < lo, q + action > hi
                 action[below | above] = 0
                 q = np.where(below, lo, np.where(above, hi, q))
-                q = q + action
+                if trem is None:
+                    q = q + action
+                else:
+                    target = np.where(trem, target + action, target)
+                    q = np.where(trem, target + wobble, q + action)
+            if trem is not None:
+                agent.target_joint_angles = target
             agent.control(agent.controllable_joint_indices, q, gains[i], forces[i])
         if step_sim:
             for _ in range(self.frame_skip):
@@ -202,6 +223,8 @@ class AssistiveEnv(gym.Env):
                     if isinstance(agent, Human):
                         agent.enforce_joint_limits()
                         if agent.controllable:                   # env.py:230-231
+                            if agent.impairment == 'tremor':     # its motors drive past the limits: the clamp moves links, at
+                                self.id.forward_kinematics()     # once as PyBullet's resetJointState does, before they are read
                             agent.enforce_realistic_joint_limits(getattr(agent, 'env_mask', None))
                 self.update_targets()
 
@@ -225,6 +248,34 @@ class AssistiveEnv(gym.Env):
             h = type(self.human)(self.human.controllable_joint_indices, controllable=self.human.controllable)
             h.init(hb, self.id, self.np_random, self.human.controllable_joint_indices)
             self.humans[g] = h
+
+    def _person_sample(self, batch, rng, *args):
+        """The reset's sample with `human_impairment` given, else None (the batch's reset draws it, as it always has).  The batch
+        draws its sample as without the keyword; then each env's impairment is drawn anew as human.py:80-92 does, and with it the
+        `limits` scale, the `weakness` strength and the tremor amplitudes (+-20 deg with the head controllable, +-10 deg for an
+        arm, stored at fp32, the precision the device keeps).  Those draws come from a stream jumped ahead of the reset's
+        generator, which they leave untouched: for a seed, gender, poses and robot placement are those of the default draw."""
+        mode = self.human_impairment_coop
+        if mode is None:
+            return None
+        s = batch.sample(self.n_envs, rng, *args)
+        g = np.random.Generator(rng.bit_generator.jumped())
+        n, k = self.n_envs, len(self.human.controllable_joint_indices)
+        amp = np.deg2rad(20 if Human.head in self.human.controllable_joint_indices else 10)
+        imp = g.integers(0, 4, size=n) if mode == 'random' else np.full(n, IMPAIRMENTS.index(mode))
+        return dict(s, impairment=imp.astype(np.int32), limit_scale=np.where(imp == 1, g.uniform(0.5, 1.0, size=n), 1.0),
+                    strength=np.where(imp == 2, g.uniform(0.25, 1.0, size=n), 1.0),
+                    tremors=np.where((imp == 3)[:, None], g.uniform(-amp, amp, size=(n, k)).astype(np.float32).astype(np.float64), 0.0))
+
+    def _person_tremor(self, s, target):
+        """The per-call side of a controllable tremor person: each gender instance's tremor mask and amplitudes, and
+        target_joint_angles [n, k] as setup_joints takes them at reset (human.py:123)."""
+        tremor = np.asarray(s['impairment']) == 3
+        for g, h in self.humans.items():
+            h.tremor_mask = tremor & (self.male if g == 'male' else ~self.male)
+            h.impairment = 'tremor' if h.tremor_mask.any() else 'none'
+            h.tremors = np.where(h.tremor_mask[:, None], s['tremors'], 0.0)
+            h.target_joint_angles = np.array(target, dtype=np.float64)
 
     def _controllable_person(self, limit_scale):
         """Both gender instances of the person act; the switched-off one moves nothing (env.py:130).  `limit_scale`: the per-env

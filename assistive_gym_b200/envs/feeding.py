@@ -27,8 +27,8 @@ def feeding_batch_for(robot):
 
 
 class FeedingEnv(AssistiveEnv):
-    def __init__(self, robot, human, n_envs=1, device=0, seed=1001, config=None):
-        super().__init__(robot=robot, human=human, task='feeding', n_envs=n_envs, device=device, seed=seed,
+    def __init__(self, robot, human, n_envs=1, device=0, seed=1001, config=None, human_impairment=None):
+        super().__init__(robot=robot, human=human, task='feeding', n_envs=n_envs, device=device, seed=seed, human_impairment=human_impairment,
                          obs_robot_len=(18 + len(robot.controllable_joint_indices) - (len(robot.wheel_joint_indices) if robot.mobile else 0)),
                          obs_human_len=(19 + len(human.controllable_joint_indices)))
         self._fb = feeding_batch_for(robot)
@@ -55,8 +55,9 @@ class FeedingEnv(AssistiveEnv):
         self.robot.motor_gains = self.human.motor_gains = 0.025          # feeding.py:122
         self.agents = [self.robot]
         coop = bool(self.human.controllable)
-        # (co-optimisation: the reference may also draw `tremor` for a controllable person, human.py:80-81; not combined here)
-        s = fb.reset(self.id, rng, settle_steps=25, impairment='no_tremor' if coop else self.human_impairment, simulate_head=coop)
+        # co-optimisation: 'no_tremor' unless `human_impairment` is given (AssistiveEnv._person_sample)
+        imp = 'no_tremor' if coop else self.human_impairment
+        s = fb.reset(self.id, rng, settle_steps=25, sample=self._person_sample(fb, rng, imp), impairment=imp, simulate_head=coop)
         self.male = s['male'].astype(bool)
         self.human.gender = 'male' if self.male[0] else 'female'
         # impairments (human.py:79-92).  The reference appends a tremor human to `agents`
@@ -72,7 +73,7 @@ class FeedingEnv(AssistiveEnv):
             h.tremors = np.where(h.tremor_mask[:, None], s['tremors'], 0.0)
             h.target_joint_angles = rest
             h.motor_gains = self.human.motor_gains
-            if h.tremor_mask.any():
+            if h.tremor_mask.any() and not coop:         # a controllable person is an agent anyway, below
                 self.agents.append(h)
         if coop:                                  # both gender instances act; the switched-off one moves nothing (env.py:130)
             for h in self.humans.values():

@@ -19,9 +19,9 @@ class FeedingJacoHumanEnv(FeedingEnv):
     {'robot': a7, 'human': a4} and returns dict observations / rewards / dones, as RLlib's MultiAgentEnv expects (learn.py:41-59).
     The person's four head joints are simulated in every env; this path goes through the per-call API (take_step + _get_obs)."""
 
-    def __init__(self, n_envs=1, device=0, seed=1001, config=None):
+    def __init__(self, n_envs=1, device=0, seed=1001, config=None, human_impairment=None):
         super().__init__(robot=Jaco(robot_arm), human=Human(human_controllable_joint_indices, controllable=True),
-                         n_envs=n_envs, device=device, seed=seed, config=config)
+                         n_envs=n_envs, device=device, seed=seed, config=config, human_impairment=human_impairment)
 
 
 class FeedingSawyerEnv(FeedingEnv):
@@ -43,14 +43,14 @@ class FeedingPR2Env(FeedingEnv):
 class FeedingSawyerHumanEnv(FeedingEnv):
     """`assistive_gym:FeedingSawyerHuman-v1` (reference envs/feeding_envs.py:51-54): as FeedingJacoHuman-v1, with Sawyer."""
 
-    def __init__(self, n_envs=1, device=0, seed=1001, config=None):
+    def __init__(self, n_envs=1, device=0, seed=1001, config=None, human_impairment=None):
         super().__init__(robot=Sawyer(robot_arm), human=Human(human_controllable_joint_indices, controllable=True),
-                         n_envs=n_envs, device=device, seed=seed, config=config)
+                         n_envs=n_envs, device=device, seed=seed, config=config, human_impairment=human_impairment)
 
 
 class FeedingPR2HumanEnv(FeedingEnv):
     """`assistive_gym:FeedingPR2Human-v1` (reference envs/feeding_envs.py:41-44): as FeedingJacoHuman-v1, with PR2's right arm."""
 
-    def __init__(self, n_envs=1, device=0, seed=1001, config=None):
+    def __init__(self, n_envs=1, device=0, seed=1001, config=None, human_impairment=None):
         super().__init__(robot=PR2(robot_arm), human=Human(human_controllable_joint_indices, controllable=True),
-                         n_envs=n_envs, device=device, seed=seed, config=config)
+                         n_envs=n_envs, device=device, seed=seed, config=config, human_impairment=human_impairment)

@@ -25,8 +25,8 @@ def scratch_batch_for(robot):
 
 
 class ScratchItchEnv(AssistiveEnv):
-    def __init__(self, robot, human, n_envs=1, device=0, seed=1001, config=None):
-        super().__init__(robot=robot, human=human, task='scratch_itch', n_envs=n_envs, device=device, seed=seed,
+    def __init__(self, robot, human, n_envs=1, device=0, seed=1001, config=None, human_impairment=None):
+        super().__init__(robot=robot, human=human, task='scratch_itch', n_envs=n_envs, device=device, seed=seed, human_impairment=human_impairment,
                          obs_robot_len=(23 + len(robot.controllable_joint_indices) - (len(robot.wheel_joint_indices) if robot.mobile else 0)),
                          obs_human_len=(24 + len(human.controllable_joint_indices)))
         self._sb = scratch_batch_for(robot)
@@ -113,7 +113,7 @@ class ScratchItchEnv(AssistiveEnv):
             self._attach(sb, sb.wheelchair, BatchSim)
         rng = np.random.default_rng(self.np_random.randint(0, 2 ** 31 - 1))
         self.agents = [self.robot]
-        s = sb.reset(self.id, rng)
+        s = sb.reset(self.id, rng, sample=self._person_sample(sb, rng))
         self.male = s['male'].astype(bool)
         self.human.gender = 'male' if self.male[0] else 'female'
         self.prev_target_contact_pos = np.zeros((self.n_envs, 3))         # scratch_itch.py:96
@@ -122,6 +122,8 @@ class ScratchItchEnv(AssistiveEnv):
             for h in self.humans.values():
                 h.enforce_joint_limits(h.controllable_joint_indices)              # the start pose is clipped to them (human.py:115 set_joint_angles)
             self.id.forward_kinematics()
+            if self.human_impairment_coop is not None:
+                self._person_tremor(s, sb.coop_tremor_target(s))
         self._limb_links, self._target_local = sb.limb_links(s), s['target_local']
         sb.start_fused(self.id, s)
         if self.human.controllable:

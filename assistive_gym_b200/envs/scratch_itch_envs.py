@@ -19,9 +19,9 @@ class ScratchItchJacoHumanEnv(ScratchItchEnv):
     {'robot': a7, 'human': a10} and returns dict observations / rewards / dones (RLlib MultiAgentEnv shape, learn.py:41-59).  The
     person's right arm is driven by its action and kept inside the realistic joint limits; per-call API path."""
 
-    def __init__(self, n_envs=1, device=0, seed=1001, config=None):
+    def __init__(self, n_envs=1, device=0, seed=1001, config=None, human_impairment=None):
         super().__init__(robot=Jaco(robot_arm), human=Human(human_controllable_joint_indices, controllable=True),
-                         n_envs=n_envs, device=device, seed=seed, config=config)
+                         n_envs=n_envs, device=device, seed=seed, config=config, human_impairment=human_impairment)
 
 
 class ScratchItchSawyerEnv(ScratchItchEnv):
@@ -43,14 +43,14 @@ class ScratchItchPR2Env(ScratchItchEnv):
 class ScratchItchSawyerHumanEnv(ScratchItchEnv):
     """`assistive_gym:ScratchItchSawyerHuman-v1` (reference envs/scratch_itch_envs.py:51-54): as ScratchItchJacoHuman-v1, with Sawyer."""
 
-    def __init__(self, n_envs=1, device=0, seed=1001, config=None):
+    def __init__(self, n_envs=1, device=0, seed=1001, config=None, human_impairment=None):
         super().__init__(robot=Sawyer(robot_arm), human=Human(human_controllable_joint_indices, controllable=True),
-                         n_envs=n_envs, device=device, seed=seed, config=config)
+                         n_envs=n_envs, device=device, seed=seed, config=config, human_impairment=human_impairment)
 
 
 class ScratchItchPR2HumanEnv(ScratchItchEnv):
     """`assistive_gym:ScratchItchPR2Human-v1` (reference envs/scratch_itch_envs.py:41-44): as ScratchItchJacoHuman-v1, with PR2's left arm."""
 
-    def __init__(self, n_envs=1, device=0, seed=1001, config=None):
+    def __init__(self, n_envs=1, device=0, seed=1001, config=None, human_impairment=None):
         super().__init__(robot=PR2(robot_arm), human=Human(human_controllable_joint_indices, controllable=True),
-                         n_envs=n_envs, device=device, seed=seed, config=config)
+                         n_envs=n_envs, device=device, seed=seed, config=config, human_impairment=human_impairment)

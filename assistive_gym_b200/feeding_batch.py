@@ -169,8 +169,18 @@ class FeedingBatch:
     def start_coop(self, sim, sample=None):
         """Arm the person's half of the fused co-optimisation step (FeedingJacoHuman-v1); call after `start_fused`.  The head
         joints are driven with the gains take_step re-issues every step (feeding.py:122: 0.025, human.py force 1.0); the
-        feeding person's limits are not scaled."""
+        feeding person's limits are not scaled.  A tremor person's head is driven by the co-optimisation step: the task's own
+        tremor, which `start_fused` arms for the same envs, is switched off."""
+        s = sample or self.last_sample
         sim.coop_init(coop_params(self.scene, self.humans, 0, TREMOR_JOINTS, 0.025))
+        imp = s.get('impairment')
+        if imp is not None and np.any(imp == 3):       # a tremor person (human_impairment given to the env)
+            sim.feeding_set_tremor(np.zeros(sim.n, dtype=np.int32), np.zeros((sim.n, 4)), np.zeros((sim.n, 4)))
+            sim.coop_set_tremor(imp == 3, self.coop_tremor_target(s), s['tremors'])
+
+    def coop_tremor_target(self, s):
+        """target_joint_angles [n, 4] of a controllable tremor person: the head pose of setup_joints (human.py:123)"""
+        return self.tremor_rest_of(s)
 
     def tremor_rest_of(self, s):
         """target_joint_angles of the head joints (human.py:122): neck 0, head x/y/z the sampled pose, limit-clipped."""

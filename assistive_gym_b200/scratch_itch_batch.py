@@ -5,7 +5,7 @@ Restates `ScratchItchEnv.reset` (reference envs/scratch_itch.py:93-153) and what
 right arm is simulated and held by weak position motors), `Tool.init` (agents/tool.py:10-47: scratcher/tool_scratch.urdf on a
 fixed constraint to the Jaco tool joint), `init_robot_pose` -> `Robot.ik_random_restarts` (envs/env.py:276-310), `generate_target`
 (scratch_itch.py:134-147, util.point_on_capsule util.py:58-78).  As in the other tasks both genders are instantiated and one
-is switched off per env; the person's `tremor` impairment is not drawn for this task, `weakness` scales the arm's motor force."""
+is switched off per env; the person's `tremor` impairment is not drawn by default (a controllable person's with `human_impairment`, `start_coop`), `weakness` scales the arm's motor force."""
 import numpy as np
 
 from . import capi
@@ -198,3 +198,21 @@ class ScratchItchBatch:
         P = coop_params(self.scene, self.humans, 1, RIGHT_ARM_JOINTS, 0.05)
         w = pack_mlp(P, load_model(), R_ARM_LIMIT_JOINTS, -1.0)
         sim.coop_init(P, limit_scale=s.get('limit_scale'), mlp=w)
+        imp = s.get('impairment')
+        if imp is not None and np.any(imp == 3):       # a tremor person (human_impairment given to the env)
+            sim.coop_set_tremor(imp == 3, self.coop_tremor_target(s), s['tremors'])
+
+    def coop_tremor_target(self, s):
+        """target_joint_angles [n, 10] of a controllable tremor person (human.py:123): the right arm's preset, clipped to the
+        limits; a tremor person's limits are not scaled, so ScratchItchEnv.reset's clip leaves it as it is"""
+        male = s['male'].astype(bool)
+        out = np.zeros((len(male), len(RIGHT_ARM_JOINTS)))
+        for g, hb in self.humans.items():
+            nj = int(self.scene['body_nlinks'][hb]) - 1
+            links = [self.gl(hb, j) for j in range(nj)]
+            q = np.zeros(nj)
+            for j, deg in HUMAN_PRESET.items():
+                q[j] = np.deg2rad(deg)
+            q = np.clip(q, self.scene['link_lower'][links], self.scene['link_upper'][links])
+            out[male if g == 'male' else ~male] = q[RIGHT_ARM_JOINTS]
+        return out

@@ -329,6 +329,14 @@ class BatchSim:
         w = None if mlp is None else np.ascontiguousarray(mlp, dtype=np.float32)
         self._ck(self.lib.ag_coop_init(self.h, C.byref(params), _p(ls), _p(w)))
 
+    def coop_set_tremor(self, on, target=None, amplitude=None):
+        """the person's tremor (after coop_init): on [n] (None = off), target and amplitude [n, n_ctrl]"""
+        k = int(self._coop_params.n_ctrl)
+        o = None if on is None else _i32(np.broadcast_to(np.asarray(on, dtype=np.int32), (self.n,)))
+        t = None if target is None else np.ascontiguousarray(np.broadcast_to(np.asarray(target, dtype=np.float64), (self.n, k)))
+        a = None if amplitude is None else _f32(amplitude, (self.n, k))
+        self._ck(self.lib.ag_coop_set_tremor(self.h, _p(o), _p(t), _p(a)))
+
     def coop_step_host(self, action):
         """action [n, 7 + n_ctrl] (robot, then person) -> obs_robot, obs_human, reward, done, info [n, 4]"""
         return self._step_host(_TASKS[int(self._coop_params.task)], action, coop=True)

@@ -401,6 +401,12 @@ typedef struct AgCoopParams {
  * NULL (classifier off).  Resets the per-env last reachable arm pose to "none yet" and sets the person's controllable motors
  * to motor_gain / motor_force (kd 1) in both genders. */
 int ag_coop_init(AgSim* sim, const AgCoopParams* p, const double* limit_scale, const float* mlp);
+/* The person's `tremor` impairment (human.py:80-92, env.py:205-215), after ag_coop_init (which switches it off): on [N] (NULL = off
+ * everywhere), target [N][n_ctrl] the envs' start target_joint_angles (human.py:123), amplitude [N][n_ctrl] the tremors.  In a
+ * tremor env the person's action accumulates into the target and the motors are driven to target +- amplitude, the sign flipping
+ * with the task's step counter.  Refused while the task's own tremor (ag_feeding_set_tremor / ag_dressing_set_tremor) is on: only
+ * one of them drives the person's joints; a coop step with both on is refused too. */
+int ag_coop_set_tremor(AgSim* sim, const int32_t* on, const double* target, const float* amplitude);
 /* action [N][7 + n_ctrl] (robot, then person); obs_robot [N][25 | 30 | 24 | 24], obs_human [N][23 | 34 | 28 | 28] for tasks 0-3,
  * reward [N], done [N], info [N][4] as the task's own step reports them.  Task 3 refuses a half-done stepSimulation, as
  * ag_dressing_step does. */
